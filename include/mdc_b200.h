@@ -215,8 +215,8 @@ int mdc_seq_prepare(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned
  * vignetteCalib optimiser, main_vignetteCalib.cpp:395-585 (SURVEY.md §8f N4).  Everything is device-resident, contiguous:
  *   d_images [n][wI*hI] float (NaN = invalidated pixel, :300-310), d_p2x / d_p2y [n][gw*gh] float plane-to-image maps
  *   (NaN = plane point not visible; finite entries keep the four bilinear taps inside the image, :352-356),
- *   d_plane_color [gw*gh], d_vignette [wI*hI].  The aruco / homography front end stays with the caller; the maps are
- *   distortCoordinates of the projected grid (mdc_fov_distort_coordinates_device).
+ *   d_plane_color [gw*gh], d_vignette [wI*hI].  The marker detection and cv::findHomography stay with the caller; the maps and
+ *   images come from mdc_vc_plane_maps and mdc_vc_prepare_images below.
  * Unlike the reference, which reads planeColor uninitialised in its first pass (:381, :425), the caller provides it.
  * integer_abs: the reference's outlier test is `abs(residual) > oth2` on a double (:423, :481).  1 = the residual is truncated to
  *   int first, which is what that line does when only `int abs(int)` is visible to unqualified lookup (libstdc++ before GCC 6,
@@ -241,6 +241,32 @@ int mdc_vc_smooth(mdc_ctx* c, const float* d_vignette, int wI, int hI, int itera
 int mdc_vignette_calib(mdc_ctx* c, const float* d_images, const float* d_p2x, const float* d_p2y, int n, int gw, int gh, int wI, int hI,
                        int max_iterations, int outlier_th, int integer_abs, float* d_plane_color, float* d_vignette, float* d_smoothed,
                        double* log_host);
+
+/* The front end in front of that loop, on the device.
+ *
+ * mdc_vc_plane_maps replaces main_vignetteCalib.cpp:266-284 followed by :346-357: for each image i the gw x gh plane grid is
+ * projected through H_i * K_p2idx^-1 (K_p2idx of :195-200 from gw, gh, facw, fach), distorted with the rectifier's
+ * distortCoordinates and masked: a point whose `int(X + 0.5)`, `int(Y + 0.5)` is not strictly inside (1, wI-2) x (1, hI-2), with
+ * wI x hI the rectifier's INPUT size, becomes NaN in both maps.  homographies: HOST doubles, [n][9] row-major as cv::findHomography
+ * returns them; d_p2x / d_p2y: DEVICE [n][gw*gh].  The 3x3 products are computed on the host in float the way the stand-in Eigen
+ * of the runnable reference program does them (inverse by adjugate / determinant); real Eigen may differ in the last bit there.
+ * Everything after that is bit-identical to the reference.  One kernel; `device` and `stream` as for
+ * mdc_fov_distort_coordinates_device.  MDC_ERR_INVALID_OBJECT (with the reference's message) for an invalid rectifier. */
+int mdc_vc_plane_maps(const mdc_fov* fov, const double* homographies, int n, int gw, int gh, float facw, float fach, float* d_p2x,
+                      float* d_p2y, int device, mdc_stream stream);
+/* mdc_vc_prepare_images replaces :286-301: image = (mean_exposure * raw) / t in fp32 (an exposure t == 0 counts as 1, :286), then
+ * the gradient invalidation: centres 2 <= x < wI-2, 2 <= y < hI-2 in raster order, neighbours deltax-major; |centre - neighbour|
+ * > max_abs_grad (the reference: 255) sets both to NaN, in place.  Bit-identical to the reference, order dependence included.
+ *   d_raw     DEVICE [n][wI*hI]: what getImage(i, false, true, false, false) gives, i.e. mdc_unmap_u8 with MDC_REMOVE_GAMMA
+ *   d_images  DEVICE [n][wI*hI] output; d_images == d_raw is allowed
+ *   exposures_host  HOST [n] exposure times of the images
+ *   mean_exposure   the caller's, computed as at :222-227: the float sum of getExposure(i) over every skip-th frame i, divided
+ *                   by getNumImages() (ALL frames, not the number summed), and 1 if that is 0.  Frames without a marker are not
+ *                   prepared (:240) but still count in the sum.
+ * Images narrower or lower than 5 pixels have no centres: normalisation only.  Any n; no host synchronisation per image.
+ * `stream` NULL = the context's stream, synchronised before returning. */
+int mdc_vc_prepare_images(mdc_ctx* c, const float* d_raw, int n, int wI, int hI, const float* exposures_host, float mean_exposure,
+                          int max_abs_grad, float* d_images, mdc_stream stream);
 
 /* responseCalib E-step, main_responseCalib.cpp:317-346 (kernel K3):
  *   d_data [n][npix] u8 image-major, d_t [n] f64 exposure times, d_G [256] f64 -> d_E [npix] f64.

@@ -49,6 +49,8 @@ SIGNATURES = {
     "mdc_vc_vignette_step": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _vp, _vp, C.c_double, C.c_int, C.POINTER(C.c_double)]),
     "mdc_vc_smooth": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, _vp]),
     "mdc_vignette_calib": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp, C.POINTER(C.c_double)]),
+    "mdc_vc_plane_maps": (C.c_int, [_vp, C.POINTER(C.c_double), C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, _vp, _vp, C.c_int, _vp]),
+    "mdc_vc_prepare_images": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, _f32p, C.c_float, C.c_int, _vp, _vp]),
     "mdc_atanf_device": (C.c_int, [_vp, _vp, C.c_size_t, C.c_int, _vp]),
     "mdc_fov_remap_x": (_f32p, [_vp]),
     "mdc_fov_remap_y": (_f32p, [_vp]),

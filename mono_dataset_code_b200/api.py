@@ -126,6 +126,18 @@ class UndistorterFOV:
         if rc not in (0, 4):        # 4 = MDC_ERR_INVALID_OBJECT: printed, like the reference
             check(rc, "mdc_fov_distort_coordinates_device")
 
+    def vcPlaneMaps(self, homographies, gw: int, gh: int, p2x, p2y, facw: float = 5.0, fach: float = 5.0) -> None:
+        """vignetteCalib's plane-to-image maps (main_vignetteCalib.cpp:266-284, :346-357) on the GPU: homographies float64 [n, 9]
+        (or [n, 3, 3]) host array; p2x / p2y float32 CUDA tensors [n, gw*gh], overwritten (NaN = not visible)."""
+        import torch
+        H = np.ascontiguousarray(homographies, np.float64).reshape(-1, 9)
+        n = H.shape[0]
+        for t_ in (p2x, p2y):
+            assert t_.is_cuda and t_.dtype == torch.float32 and t_.is_contiguous() and tuple(t_.shape) == (n, gw * gh)
+        check(lib.mdc_vc_plane_maps(self._h, H.ctypes.data_as(C.POINTER(C.c_double)), n, gw, gh, float(facw), float(fach),
+                                    C.c_void_p(p2x.data_ptr()), C.c_void_p(p2y.data_ptr()), p2x.device.index or 0,
+                                    Context._stream(p2x)), "mdc_vc_plane_maps")
+
     # ---- per-frame operator (FOVUndistorter.cpp:322-370)
     def _context(self, device=0):
         if self._ctx is None:
@@ -390,6 +402,20 @@ class Context:
         for t_, cols in ((images, wI * hI), (p2x, gw * gh), (p2y, gw * gh)):
             assert t_.is_cuda and t_.dtype == torch.float32 and t_.is_contiguous() and tuple(t_.shape) == (n, cols)
         return n
+
+    def vc_prepare_images(self, raw, wI, hI, exposures, mean_exposure, max_abs_grad=255, out=None):
+        """Exposure normalisation + gradient invalidation (main_vignetteCalib.cpp:286-301): raw float32 CUDA tensor [n, wI*hI],
+        exposures [n] (host); out defaults to a new tensor and may be raw itself.  Returns out."""
+        import torch
+        n = raw.shape[0]
+        out = torch.empty_like(raw) if out is None else out
+        for t_ in (raw, out):
+            assert t_.is_cuda and t_.dtype == torch.float32 and t_.is_contiguous() and tuple(t_.shape) == (n, wI * hI)
+        t = np.ascontiguousarray(np.asarray(exposures, np.float32).reshape(-1))
+        assert t.size == n
+        check(lib.mdc_vc_prepare_images(self._h, C.c_void_p(raw.data_ptr()), n, wI, hI, t.ctypes.data_as(_f32p), float(mean_exposure),
+                                        int(max_abs_grad), C.c_void_p(out.data_ptr()), self._stream(raw)), "mdc_vc_prepare_images")
+        return out
 
     def vc_plane_step(self, images, p2x, p2y, gw, gh, wI, hI, vignette, plane_color, oth2, integer_abs=True):
         """plane_color is updated in place; returns (E, R)."""

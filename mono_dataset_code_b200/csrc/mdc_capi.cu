@@ -910,6 +910,36 @@ extern "C" int mdc_fov_distort_coordinates_device(const mdc_fov* f, float* d_x, 
     return MDC_OK;
 }
 
+extern "C" int mdc_vc_plane_maps(const mdc_fov* fov, const double* homographies, int n, int gw, int gh, float facw, float fach, float* d_p2x,
+                                 float* d_p2y, int device, mdc_stream stream) {
+    if (!fov || n < 0 || gw < 0 || gh < 0 || (n && (!homographies || (static_cast<size_t>(gw) * gh && (!d_p2x || !d_p2y))))) {
+        mdc_set_error("mdc_vc_plane_maps: bad argument");
+        return MDC_ERR_INVALID_ARG;
+    }
+    if (!fov->valid) {
+        printf("ERROR: invalid UndistorterFOV!\n");          // distortCoordinates, FOVUndistorter.cpp:282-286
+        mdc_set_error("mdc_vc_plane_maps on an invalid rectifier");
+        return MDC_ERR_INVALID_OBJECT;
+    }
+    if (n == 0 || static_cast<size_t>(gw) * gh == 0) return MDC_OK;
+    std::vector<float> hk(static_cast<size_t>(9) * n);
+    for (int i = 0; i < n; ++i) mdc_vc_plane_matrix(homographies + 9 * static_cast<size_t>(i), gw, gh, facw, fach, hk.data() + 9 * static_cast<size_t>(i));
+    mdc_distort_constants h;
+    mdc_fov_distort_constants(fov, &h);
+    const DistortConstants k{h.ocx, h.ocy, h.ofx, h.ofy, h.d2t, h.omega, h.fx, h.fy, h.cx, h.cy};
+    CU_CHECK(cudaSetDevice(device));
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    float* d_hk = nullptr;
+    CU_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&d_hk), hk.size() * sizeof(float), s));
+    cudaError_t e = cudaMemcpyAsync(d_hk, hk.data(), hk.size() * sizeof(float), cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = launch_vc_plane_maps(d_hk, n, gw, gh, fov->in_w, fov->in_h, k, d_p2x, d_p2y, s);
+    const cudaError_t f = cudaFreeAsync(d_hk, s);
+    CU_CHECK(e);
+    CU_CHECK(f);
+    if (!stream) CU_CHECK(cudaStreamSynchronize(nullptr));
+    return MDC_OK;
+}
+
 extern "C" int mdc_atanf_device(const float* d_in, float* d_out, size_t n, int device, mdc_stream stream) {
     if (n && (!d_in || !d_out)) { mdc_set_error("mdc_atanf_device: bad argument"); return MDC_ERR_INVALID_ARG; }
     CU_CHECK(cudaSetDevice(device));

@@ -106,6 +106,26 @@ void mdc_fov_distort(const mdc_fov* f, float* xs, float* ys, int n) {
     }
 }
 
+// HK = H * K_p2idx^-1 of main_vignetteCalib.cpp:195-200, :254-271, in float with the arithmetic of the stand-in Eigen the runnable
+// reference program is built against (oracle/shim/Eigen/Core): inverse by adjugate / determinant, product summed left to right.
+// Real Eigen may order the inverse differently and differ in the last bit.
+void mdc_vc_plane_matrix(const double H[9], int gw, int gh, float facw, float fach, float HK[9]) {
+    float K[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, Ki[9], Hf[9];
+    K[0] = gw / facw; K[4] = gh / fach; K[2] = gw / 2; K[5] = gh / 2; K[8] = 1;      // gw / 2 is an int division
+    const float c00 = K[4] * K[8] - K[5] * K[7], c01 = K[5] * K[6] - K[3] * K[8], c02 = K[3] * K[7] - K[4] * K[6];
+    const float det = K[0] * c00 + K[1] * c01 + K[2] * c02;
+    Ki[0] = c00 / det; Ki[3] = c01 / det; Ki[6] = c02 / det;
+    Ki[1] = (K[2] * K[7] - K[1] * K[8]) / det;
+    Ki[4] = (K[0] * K[8] - K[2] * K[6]) / det;
+    Ki[7] = (K[1] * K[6] - K[0] * K[7]) / det;
+    Ki[2] = (K[1] * K[5] - K[2] * K[4]) / det;
+    Ki[5] = (K[2] * K[3] - K[0] * K[5]) / det;
+    Ki[8] = (K[0] * K[4] - K[1] * K[3]) / det;
+    for (int i = 0; i < 9; ++i) Hf[i] = static_cast<float>(H[i]);          // Eigen::Matrix3f H from the double cv::Mat, :255-263
+    for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) HK[r * 3 + c] = Hf[r * 3] * Ki[c] + Hf[r * 3 + 1] * Ki[3 + c] + Hf[r * 3 + 2] * Ki[6 + c];
+}
+
 // the restated atanf (mdc_atanf.h) evaluated on the host, so that it can be compared with the platform's libm without a GPU
 extern "C" void mdc_atanf_host(const float* in, float* out, size_t n) {
     for (size_t i = 0; i < n; ++i) out[i] = mdc_atanf(in[i]);

@@ -46,6 +46,7 @@ void mdc_fov_build(mdc_fov* f, int mode, const float out_calib_in[5]);
 struct mdc_distort_constants { float ocx, ocy, ofx, ofy, d2t, omega, fx, fy, cx, cy; };
 void mdc_fov_distort_constants(const mdc_fov* f, mdc_distort_constants* k);
 void mdc_fov_distort(const mdc_fov* f, float* xs, float* ys, int n);
+void mdc_vc_plane_matrix(const double H[9], int gw, int gh, float facw, float fach, float HK[9]);      // vignetteCalib's H * K_p2idx^-1
 bool mdc_photo_set_gamma(mdc_photo* p, const float raw[256]);
 void mdc_photo_set_vignette(mdc_photo* p, const void* pixels, int depth);
 

@@ -983,16 +983,50 @@ cudaError_t launch_pyr_down(const float* src, int sw, int sh, float* dst, int n_
 // distortCoordinates on the device (FOVUndistorter.cpp:280-319), in place, bit-identical to the host: explicit IEEE
 // operations in the reference's order, atanf restated from glibc (mdc_atanf.h).
 // =====================================================================================
+__device__ __forceinline__ void fov_distort_point(float& x, float& y, const DistortConstants& k) {
+    const float nx = __fdiv_rn(__fsub_rn(x, k.ocx), k.ofx);
+    const float ny = __fdiv_rn(__fsub_rn(y, k.ocy), k.ofy);
+    const float rad = __fsqrt_rn(__fadd_rn(__fmul_rn(nx, nx), __fmul_rn(ny, ny)));
+    float scale = 1.0f;
+    if (!(rad == 0.0f || k.omega == 0.0f)) scale = __fdiv_rn(mdc_atanf(__fmul_rn(rad, k.d2t)), __fmul_rn(k.omega, rad));
+    x = __fadd_rn(__fmul_rn(__fmul_rn(k.fx, scale), nx), k.cx);
+    y = __fadd_rn(__fmul_rn(__fmul_rn(k.fy, scale), ny), k.cy);
+}
 __global__ void __launch_bounds__(256) fov_distort_kernel(float* __restrict__ xs, float* __restrict__ ys, size_t n, DistortConstants k) {
     const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
     for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
-        const float nx = __fdiv_rn(__fsub_rn(xs[i], k.ocx), k.ofx);
-        const float ny = __fdiv_rn(__fsub_rn(ys[i], k.ocy), k.ofy);
-        const float rad = __fsqrt_rn(__fadd_rn(__fmul_rn(nx, nx), __fmul_rn(ny, ny)));
-        float scale = 1.0f;
-        if (!(rad == 0.0f || k.omega == 0.0f)) scale = __fdiv_rn(mdc_atanf(__fmul_rn(rad, k.d2t)), __fmul_rn(k.omega, rad));
-        xs[i] = __fadd_rn(__fmul_rn(__fmul_rn(k.fx, scale), nx), k.cx);
-        ys[i] = __fadd_rn(__fmul_rn(__fmul_rn(k.fy, scale), ny), k.cy);
+        float x = xs[i], y = ys[i];
+        fov_distort_point(x, y, k);
+        xs[i] = x;
+        ys[i] = y;
+    }
+}
+
+// vignetteCalib's plane-to-image maps (main_vignetteCalib.cpp:266-284 and :346-357) in one pass: grid point (x, y) of image img is
+// projected through hk[img] = H * K_p2idx^-1 (9 floats, row-major, built on the host), distorted, and masked.  pp[r] =
+// HK[r,0]*x + HK[r,1]*y + HK[r,2]*1 left to right, then pp[0]/pp[2], pp[1]/pp[2], as the stand-in Eigen product the reference
+// program builds against evaluates it.  The mask is `int u_d = X + 0.5` (a double add, then truncation): x86 converts NaN and
+// out-of-range values to INT_MIN, __double2int_rz saturates and turns NaN into 0; both fail `u_d > 1 && u_d < wI-2`, so the same
+// points are rejected.
+__global__ void __launch_bounds__(256) vc_plane_maps_kernel(const float* __restrict__ hk, int gw, size_t gwgh, size_t total, int wI, int hI,
+                                                            DistortConstants k, float* __restrict__ xs, float* __restrict__ ys) {
+    const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
+    for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += stride) {
+        const size_t img = i / gwgh, pt = i - img * gwgh;
+        const int gy = static_cast<int>(pt / gw), gx = static_cast<int>(pt - static_cast<size_t>(gy) * gw);
+        const float* m = hk + 9 * img;
+        const float fx = static_cast<float>(gx), fy = static_cast<float>(gy);
+        float pp[3];
+#pragma unroll
+        for (int r = 0; r < 3; ++r)
+            pp[r] = __fadd_rn(__fadd_rn(__fmul_rn(__ldg(m + 3 * r), fx), __fmul_rn(__ldg(m + 3 * r + 1), fy)), __fmul_rn(__ldg(m + 3 * r + 2), 1.0f));
+        float x = __fdiv_rn(pp[0], pp[2]), y = __fdiv_rn(pp[1], pp[2]);
+        fov_distort_point(x, y, k);
+        const int u_d = __double2int_rz(__dadd_rn(static_cast<double>(x), 0.5));
+        const int v_d = __double2int_rz(__dadd_rn(static_cast<double>(y), 0.5));
+        if (!(u_d > 1 && v_d > 1 && u_d < wI - 2 && v_d < hI - 2)) x = y = __int_as_float(0x7fc00000);
+        xs[i] = x;
+        ys[i] = y;
     }
 }
 __global__ void __launch_bounds__(256) atanf_kernel(const float* __restrict__ in, float* __restrict__ out, size_t n) {
@@ -1007,6 +1041,13 @@ static unsigned stream_blocks(size_t n) {
 cudaError_t launch_fov_distort(float* xs, float* ys, size_t n, const DistortConstants& k, cudaStream_t stream) {
     if (n == 0) return cudaSuccess;
     fov_distort_kernel<<<stream_blocks(n), 256, 0, stream>>>(xs, ys, n, k);
+    return cudaGetLastError();
+}
+cudaError_t launch_vc_plane_maps(const float* hk, int n, int gw, int gh, int wI, int hI, const DistortConstants& k, float* xs, float* ys,
+                                 cudaStream_t stream) {
+    const size_t gwgh = static_cast<size_t>(gw) * gh, total = gwgh * n;
+    if (total == 0) return cudaSuccess;
+    vc_plane_maps_kernel<<<stream_blocks(total), 256, 0, stream>>>(hk, gw, gwgh, total, wI, hI, k, xs, ys);
     return cudaGetLastError();
 }
 cudaError_t launch_atanf(const float* in, float* out, size_t n, cudaStream_t stream) {

@@ -91,6 +91,9 @@ cudaError_t launch_pyr_down2(const float* src, int sw, int sh, float* d1, float*
 struct DistortConstants { float ocx, ocy, ofx, ofy, d2t, omega, fx, fy, cx, cy; };
 cudaError_t launch_fov_distort(float* xs, float* ys, size_t n, const DistortConstants& k, cudaStream_t stream);
 cudaError_t launch_atanf(const float* in, float* out, size_t n, cudaStream_t stream);
+// vignetteCalib plane-to-image maps: hk [n][9] device floats (H * K_p2idx^-1 per image); xs/ys [n][gw*gh]
+cudaError_t launch_vc_plane_maps(const float* hk, int n, int gw, int gh, int wI, int hI, const DistortConstants& k, float* xs, float* ys,
+                                 cudaStream_t stream);
 cudaError_t launch_estep(const uint8_t* data, int n, int npix, const double* t, const double* G, double* E,
                          cudaStream_t stream);
 

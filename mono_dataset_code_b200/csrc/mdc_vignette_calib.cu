@@ -14,6 +14,8 @@
 //                             reference's chain only by the rounding error of that chain (compared to 2e-5 relative).
 //                             Then CT/TT, the maximum, the division.
 //   smoothing (:542-566)      NaN-aware 3x3 mean, ping-pong buffers, bit-identical.
+//   front end (:286-301)      exposure normalisation, then the order-dependent gradient invalidation as a flag pass plus a
+//                             skewed wavefront per image (see vc_grad_resolve_kernel), bit-identical.
 //
 // All float arithmetic is spelled out with round-to-nearest intrinsics in the reference's evaluation order (no FMA).
 #include <cuda_runtime.h>
@@ -21,6 +23,9 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
+
+#include <algorithm>
+#include <vector>
 
 #include "mdc_b200.h"
 #include "mdc_internal.h"
@@ -320,6 +325,81 @@ __global__ void __launch_bounds__(256) vc_smooth_kernel(const float* __restrict_
     }
 }
 
+// ---- front end: the images the loop works on (:286-301)
+// image = (meanExposure * raw) / exposure, elementwise (in place allowed); exposures[img] has 0 already replaced by 1 (:286)
+__global__ void __launch_bounds__(256) vc_normalise_images_kernel(const float* raw, float* out, size_t npx, size_t total,
+                                                                  const float* __restrict__ exposures, float mean_exposure) {
+    const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
+    for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += stride)
+        out[i] = __fdiv_rn(__fmul_rn(mean_exposure, raw[i]), __ldg(exposures + i / npx));
+}
+
+// The gradient invalidation (:293-301) visits the centres 2 <= x < wI-2, 2 <= y < hI-2 in raster order and compares each with its
+// 24 neighbours (deltax-major); a hit sets centre and neighbour to NaN, in place, so the result depends on the order.  Values only
+// ever become NaN and a comparison with NaN is false, so a comparison can only fire if it fires on the normalised values as they
+// are before the pass.  Pass 1 (vc_grad_flags_kernel) therefore marks, data-parallel, every centre that has at least one candidate
+// hit: one bit per centre, 32 consecutive centres of a row per word.  Pass 2 (vc_grad_resolve_kernel) replays the reference's loop
+// literally, on the current values, at the marked centres only, in an order that is equivalent to raster order: the centre at
+// (x, y) runs at step x + 5y.  Two centres of one step are at least 5 columns apart, so their 5x5 windows are disjoint; a centre
+// whose window overlaps that of an earlier centre in raster order (|dx| <= 4, |dy| <= 4) runs at a strictly earlier step.  Each
+// step is one __syncthreads apart, and the pixels live in global memory (one CTA per image: the writes of a step are visible to
+// the whole CTA after the barrier).
+__device__ __forceinline__ bool vc_grad_hit(float c, float nb, float g) { return fabsf(__fsub_rn(c, nb)) > g; }
+
+// one thread per centre column x of a 32-wide word (x = word*32 + lane); the words of row y: flags[img][y][0 .. words)
+__global__ void __launch_bounds__(256) vc_grad_flags_kernel(const float* __restrict__ images, int wI, int hI, int words, size_t total,
+                                                            float g, unsigned* __restrict__ flags) {
+    const size_t npx = static_cast<size_t>(wI) * hI;
+    const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;      // total and stride are multiples of 32: whole warps
+    for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += stride) {
+        const size_t row = i >> 5;                          // img * hI + y
+        const int word = static_cast<int>(row % words);
+        const size_t img_y = row / words;
+        const int y = static_cast<int>(img_y % hI);
+        const size_t img = img_y / hI;
+        const int x = word * 32 + static_cast<int>(i & 31);
+        bool hit = false;
+        if (x >= 2 && x < wI - 2 && y >= 2 && y < hI - 2) {
+            const float* p = images + img * npx + static_cast<size_t>(y) * wI + x;
+            const float c = __ldg(p);
+            for (int dy = -2; dy <= 2 && !hit; ++dy)
+                for (int dx = -2; dx <= 2; ++dx)
+                    if (vc_grad_hit(c, __ldg(p + dy * wI + dx), g)) { hit = true; break; }
+        }
+        const unsigned bits = __ballot_sync(0xffffffffu, hit);
+        if ((i & 31) == 0) flags[row] = bits;
+    }
+}
+
+// one CTA per image of the chunk; at step t the centres x + 5y = t run, one per row, rows spread over the CTA's threads
+__global__ void __launch_bounds__(256) vc_grad_resolve_kernel(float* images, int wI, int hI, int words, float g, const unsigned* __restrict__ flags) {
+    float* im = images + static_cast<size_t>(blockIdx.x) * wI * hI;
+    const unsigned* fl = flags + static_cast<size_t>(blockIdx.x) * hI * words;
+    const int t_last = (wI - 3) + 5 * (hI - 3);
+    for (int t = 2 + 5 * 2; t <= t_last; ++t) {
+        // rows y with 2 <= x = t - 5y <= wI-3 and 2 <= y <= hI-3
+        const int lo = max(2, (t - (wI - 3) + 4) / 5), hi = min(hI - 3, (t - 2) / 5);
+        for (int y = lo + static_cast<int>(threadIdx.x); y <= hi; y += blockDim.x) {
+            const int x = t - 5 * y;
+            if (!((__ldg(fl + static_cast<size_t>(y) * words + (x >> 5)) >> (x & 31)) & 1u)) continue;
+            float* p = im + static_cast<size_t>(y) * wI + x;
+            // the reference's loop (:296-300) on the current values; once the centre is NaN no comparison can fire
+            bool dead = false;
+            for (int dx = -2; dx <= 2 && !dead; ++dx)
+                for (int dy = -2; dy <= 2; ++dy) {
+                    float* q = p + dx + dy * wI;
+                    if (vc_grad_hit(*p, *q, g)) {
+                        *p = __int_as_float(0x7fc00000);
+                        *q = __int_as_float(0x7fc00000);
+                        dead = true;
+                        break;
+                    }
+                }
+        }
+        __syncthreads();
+    }
+}
+
 unsigned vc_blocks(size_t work) {
     size_t b = (work + 255) / 256;
     if (b > static_cast<size_t>(kVcMaxBlocks)) b = kVcMaxBlocks;
@@ -463,6 +543,63 @@ extern "C" int mdc_vc_vignette_step(mdc_ctx* c, const float* d_images, const flo
     cudaFree(sc.base);
     if (stats_host) { stats_host[0] = st[0]; stats_host[1] = st[1]; }
     return rc;
+}
+
+// flags scratch of one chunk of images: at most this many bytes, and at most kVcPrepChunkImages images (one resolve CTA each)
+constexpr size_t kVcPrepScratchBytes = size_t(64) << 20;
+constexpr int kVcPrepChunkImages = 512;
+
+extern "C" int mdc_vc_prepare_images(mdc_ctx* c, const float* d_raw, int n, int wI, int hI, const float* exposures_host, float mean_exposure,
+                                     int max_abs_grad, float* d_images, mdc_stream stream) {
+    if (!c || n < 0 || wI < 0 || hI < 0 || (n && wI && hI && (!d_raw || !d_images || !exposures_host))) {
+        mdc_set_error("mdc_vc_prepare_images: bad argument");
+        return MDC_ERR_INVALID_ARG;
+    }
+    const size_t npx = static_cast<size_t>(wI) * hI;
+    if (n == 0 || npx == 0) return MDC_OK;
+    VC_CHECK(cudaSetDevice(mdc_ctx_device_ordinal(c)));
+    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : static_cast<cudaStream_t>(mdc_ctx_stream_handle(c));
+    std::vector<float> t(exposures_host, exposures_host + n);
+    for (float& e : t)
+        if (e == 0) e = 1;                                   // :286
+    const bool has_centres = wI >= 5 && hI >= 5;
+    const int words = (wI + 31) / 32;
+    const size_t flag_bytes = static_cast<size_t>(hI) * words * sizeof(unsigned);
+    size_t chunk = std::min<size_t>(std::max<size_t>(kVcPrepScratchBytes / flag_bytes, 1), kVcPrepChunkImages);
+    chunk = std::min<size_t>(chunk, static_cast<size_t>(n));
+    char* scratch = nullptr;      // exposures [n], then the flags of one chunk (256-byte aligned)
+    const size_t expo_bytes = (static_cast<size_t>(n) * sizeof(float) + 255) / 256 * 256;
+    VC_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&scratch), expo_bytes + (has_centres ? chunk * flag_bytes : 0), s));
+    const float* d_expo = reinterpret_cast<const float*>(scratch);
+    unsigned* d_flags = reinterpret_cast<unsigned*>(scratch + expo_bytes);
+    int launches = 1;
+    cudaError_t e = cudaMemcpyAsync(scratch, t.data(), static_cast<size_t>(n) * sizeof(float), cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) {
+        const size_t total = npx * n;
+        vc_normalise_images_kernel<<<vc_blocks(total), 256, 0, s>>>(d_raw, d_images, npx, total, d_expo, mean_exposure);
+        e = cudaGetLastError();
+    }
+    if (has_centres) {
+        const float g = static_cast<float>(max_abs_grad);    // fabsf(...) > maxAbsGrad compares in float (:299)
+        // threads per resolve CTA: enough for the rows one step touches (about (wI-4)/5), whole warps, at most 256
+        const int rows = std::min((wI - 4 + 4) / 5, hI - 4);
+        const int threads = std::min(256, std::max(32, (rows + 31) / 32 * 32));
+        for (size_t first = 0; first < static_cast<size_t>(n) && e == cudaSuccess; first += chunk) {
+            const size_t m = std::min(chunk, static_cast<size_t>(n) - first);
+            float* im = d_images + first * npx;
+            const size_t lanes = m * hI * words * 32;
+            vc_grad_flags_kernel<<<vc_blocks(lanes), 256, 0, s>>>(im, wI, hI, words, lanes, g, d_flags);
+            vc_grad_resolve_kernel<<<static_cast<unsigned>(m), threads, 0, s>>>(im, wI, hI, words, g, d_flags);
+            e = cudaGetLastError();
+            launches += 2;
+        }
+    }
+    const cudaError_t f = cudaFreeAsync(scratch, s);
+    mdc_ctx_add_launches(c, launches);
+    VC_CHECK(e);
+    VC_CHECK(f);
+    if (!stream) VC_CHECK(cudaStreamSynchronize(s));
+    return MDC_OK;
 }
 
 extern "C" int mdc_vc_smooth(mdc_ctx* c, const float* d_vignette, int wI, int hI, int iterations, float* d_out) {

@@ -1,0 +1,252 @@
+// vignetteCalib on the GPU: a C++ host for the front end and the optimiser behind include/mdc_b200.h.
+//
+// Same command line, inputs and result files as the reference's vignetteCalib program (main_vignetteCalib.cpp:132-180 arguments,
+// :222-227 mean exposure, :230-372 front end, :395-585 optimisation loop, :531 log.txt rows, :72-93 plane.png, :570-582
+// vignette.png / vignetteSmoothed.png), with every pass over the images and plane grids running in the sm_90a kernels of
+// libmdc_b200.so: gamma removal (mdc_unmap_u8), exposure normalisation and gradient invalidation (mdc_vc_prepare_images),
+// projection + distortion + visibility mask of the plane grid (mdc_vc_plane_maps), and the loop (mdc_vignette_calib).
+//
+// The marker detection (aruco) and cv::findHomography are not part of the library.  Their result comes from a file instead:
+// nine whitespace-separated numbers (the row-major 3x3 homography from marker corners to rectified pixels) per considered frame
+// i = 0, skip, 2*skip, ...  A row containing NaN means that no marker was found in that frame: the frame is left out (:240),
+// but its exposure still counts in the mean exposure, as in the reference.  The debug overlays and imshow windows (:306-368) are
+// not produced.
+//
+//   vignetteCalib_b200 <dataset dir/> homographies=FILE [iterations=20] [skip=1] [patternX=1000] [patternY=1000] [facW=5] [facH=5]
+//                      [device=0]
+//
+// Build (see tests/test_vignette_calib_tool.py):  g++ -std=c++11 -O2 -Iinclude tools/vignetteCalib_b200.cpp
+//                                                 -Lmono_dataset_code_b200/lib -lmdc_b200 -L/usr/local/cuda/lib64 -lcudart -lz
+#include <cuda_runtime.h>
+#include <zlib.h>
+
+#include <cmath>
+#include <cstdint>
+#include <cstdio>
+#include <cstdlib>
+#include <cstring>
+#include <fstream>
+#include <string>
+#include <vector>
+
+#include "mdc_b200.h"
+
+namespace {
+
+struct Options {
+    int iterations = 20, skip = 1, gw = 1000, gh = 1000, device = 0;
+    float facw = 5, fach = 5;
+    std::string homographies;
+};
+
+void parse_option(const char* arg, Options* o) {
+    int v;
+    float f;
+    if (strncmp(arg, "homographies=", 13) == 0) { o->homographies = arg + 13; return; }
+    if (sscanf(arg, "iterations=%d", &v) == 1) { o->iterations = v; printf("nits set to %d!\n", v); return; }
+    if (sscanf(arg, "skip=%d", &v) == 1) { o->skip = v; printf("skipFrames set to %d!\n", v); return; }
+    if (sscanf(arg, "patternX=%d", &v) == 1) { o->gw = v; printf("patternX set to %d!\n", v); return; }
+    if (sscanf(arg, "patternY=%d", &v) == 1) { o->gh = v; printf("patternY set to %d!\n", v); return; }
+    if (sscanf(arg, "facW=%f", &f) == 1) { o->facw = f; printf("facw set to %f!\n", f); return; }
+    if (sscanf(arg, "facH=%f", &f) == 1) { o->fach = f; printf("fach set to %f!\n", f); return; }
+    if (sscanf(arg, "device=%d", &v) == 1) { o->device = v; return; }
+    printf("could not parse argument \"%s\"!!\n", arg);
+}
+
+#define CUDA_OR_DIE(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) { printf("%s: %s\n", #expr, cudaGetErrorString(e__)); exit(2); } } while (0)
+#define MDC_OR_DIE(expr) do { int r__ = (expr); if (r__ != MDC_OK) { printf("%s failed (%d): %s\n", #expr, r__, mdc_last_error()); exit(2); } } while (0)
+
+// PNG with filter type 0 on every row: colour type 0 (grey) or 2 (RGB), 8 or 16 bits, samples big-endian
+bool write_png(const std::string& path, const std::vector<uint8_t>& rows_be, int w, int h, int depth, int colour) {
+    const size_t stride = static_cast<size_t>(w) * (colour == 2 ? 3 : 1) * (depth / 8);
+    std::vector<uint8_t> raw;
+    raw.reserve((stride + 1) * h);
+    for (int y = 0; y < h; ++y) {
+        raw.push_back(0);
+        raw.insert(raw.end(), rows_be.begin() + y * stride, rows_be.begin() + (y + 1) * stride);
+    }
+    uLongf zlen = compressBound(raw.size());
+    std::vector<uint8_t> z(zlen);
+    if (compress2(z.data(), &zlen, raw.data(), raw.size(), 6) != Z_OK) return false;
+    z.resize(zlen);
+    FILE* f = fopen(path.c_str(), "wb");
+    if (!f) return false;
+    auto be32 = [](uint8_t* p, uint32_t v) { p[0] = v >> 24; p[1] = v >> 16; p[2] = v >> 8; p[3] = v; };
+    auto chunk = [&](const char* tag, const uint8_t* data, size_t len) {
+        uint8_t head[8];
+        be32(head, static_cast<uint32_t>(len));
+        memcpy(head + 4, tag, 4);
+        uLong crc = crc32(0L, head + 4, 4);
+        if (len) crc = crc32(crc, data, static_cast<uInt>(len));
+        uint8_t tail[4];
+        be32(tail, static_cast<uint32_t>(crc));
+        fwrite(head, 1, 8, f);
+        if (len) fwrite(data, 1, len, f);
+        fwrite(tail, 1, 4, f);
+    };
+    static const uint8_t sig[8] = {0x89, 'P', 'N', 'G', '\r', '\n', 0x1a, '\n'};
+    fwrite(sig, 1, 8, f);
+    uint8_t ihdr[13];
+    be32(ihdr, w);
+    be32(ihdr + 4, h);
+    ihdr[8] = static_cast<uint8_t>(depth); ihdr[9] = static_cast<uint8_t>(colour); ihdr[10] = ihdr[11] = ihdr[12] = 0;
+    chunk("IHDR", ihdr, 13);
+    chunk("IDAT", z.data(), z.size());
+    chunk("IEND", nullptr, 0);
+    return fclose(f) == 0;
+}
+
+// cv::Mat(CV_32F) * 254.9 * 254.9 -> convertTo(CV_16U) (:570-581): two float products, then round to nearest even and saturate
+// (NaN -> 0)
+bool write_vignette_png(const std::string& path, const std::vector<float>& v, int w, int h) {
+    std::vector<uint8_t> px(v.size() * 2);
+    for (size_t i = 0; i < v.size(); ++i) {
+        float a = static_cast<float>(v[i] * 254.9);
+        a = static_cast<float>(a * 254.9);
+        const double r = nearbyint(static_cast<double>(a));
+        const unsigned u = r > 65535 ? 65535u : (r > 0 ? static_cast<unsigned>(r) : 0u);
+        px[2 * i] = static_cast<uint8_t>(u >> 8);
+        px[2 * i + 1] = static_cast<uint8_t>(u);
+    }
+    return write_png(path, px, w, h, 16, 0);
+}
+
+// displayImage (:72-93): grey 255*(I-vmin)/(vmax-vmin) truncated to 8 bits; NaN is the Mat's BGR (0,0,255), i.e. red
+bool write_plane_png(const std::string& path, const std::vector<float>& I, int w, int h) {
+    float vmin = 1e10, vmax = -1e10;
+    for (float v : I) {
+        if (vmin > v) vmin = v;
+        if (vmax < v) vmax = v;
+    }
+    printf("plane image values %f - %f!\n", vmin, vmax);
+    std::vector<uint8_t> px(I.size() * 3);
+    for (size_t i = 0; i < I.size(); ++i) {
+        uint8_t* p = &px[3 * i];
+        if (std::isnan(I[i])) { p[0] = 255; p[1] = 0; p[2] = 0; continue; }
+        const float c = 255 * (I[i] - vmin) / (vmax - vmin);
+        p[0] = p[1] = p[2] = c >= 0 && c < 256 ? static_cast<uint8_t>(c) : (c >= 256 ? 255 : 0);
+    }
+    return write_png(path, px, w, h, 8, 2);
+}
+
+}  // namespace
+
+int main(int argc, char** argv) {
+    if (argc < 2) {
+        printf("usage: vignetteCalib_b200 <dataset dir/> homographies=FILE [iterations=N] [skip=N] [patternX=N] [patternY=N] [facW=F] [facH=F] "
+               "[device=N]\n");
+        return 1;
+    }
+    Options opt;
+    for (int i = 2; i < argc; ++i) parse_option(argv[i], &opt);
+    if (opt.skip < 1) opt.skip = 1;
+    if (opt.homographies.empty()) { printf("homographies=FILE is required\n"); return 1; }
+    if (opt.gw < 1 || opt.gh < 1) { printf("patternX / patternY must be positive\n"); return 1; }
+
+    if (system("rm -rf vignetteCalibResult") == -1) printf("could not delete old vignetteCalibResult folder!\n");
+    if (system("mkdir vignetteCalibResult") == -1) printf("could not create vignetteCalibResult folder!\n");
+
+    // ---- the dataset as DatasetReader opens it: frames + times.txt, camera.txt, pcalib.txt + vignette.png
+    const std::string path = argv[1];
+    printf("SEQUENCE NAME: %s!\n", argv[1]);
+    mdc_seq* seq = nullptr;
+    if (mdc_seq_open(argv[1], &seq) != MDC_OK) { printf("cannot open dataset %s: %s\n", argv[1], mdc_last_error()); return 1; }
+    mdc_fov* fov = nullptr;
+    if (mdc_fov_create((path + "camera.txt").c_str(), &fov) != MDC_OK) { printf("invalid camera.txt: %s\n", mdc_last_error()); return 1; }
+    int wI = 0, hI = 0, w_out = 0, h_out = 0;
+    mdc_fov_dims(fov, &wI, &hI, &w_out, &h_out);
+    mdc_photo* photo = nullptr;
+    mdc_photo_create((path + "pcalib.txt").c_str(), (path + "vignette.png").c_str(), wI, hI, &photo);      // only the response is used
+    const int num_images = mdc_seq_num_images(seq);
+
+    // :222-227: the sum runs over every skip-th frame but is divided by the number of ALL frames
+    float mean_exposure = 0;
+    for (int i = 0; i < num_images; i += opt.skip) mean_exposure += mdc_seq_exposure(seq, i);
+    mean_exposure = mean_exposure / num_images;
+    if (mean_exposure == 0) mean_exposure = 1;
+
+    // ---- frames that have a homography
+    FILE* hf = fopen(opt.homographies.c_str(), "r");
+    if (!hf) { printf("cannot open %s\n", opt.homographies.c_str()); return 1; }
+    const size_t npx = static_cast<size_t>(wI) * hI;
+    std::vector<uint8_t> stack, frame(npx);
+    std::vector<float> exposures;
+    std::vector<double> Hs;
+    for (int i = 0; i < num_images; i += opt.skip) {
+        double H[9];
+        for (int k = 0; k < 9; ++k)
+            if (fscanf(hf, "%lf", &H[k]) != 1) { printf("%s: no homography for frame %d\n", opt.homographies.c_str(), i); return 1; }
+        bool found = true;
+        for (double v : H) found = found && !std::isnan(v);
+        if (!found) continue;                                   // no marker in this frame (:240)
+        int fw = 0, fh = 0;
+        if (mdc_seq_read_gray8(seq, i, frame.data(), frame.size(), &fw, &fh) != MDC_OK || fw != wI || fh != hI) {
+            printf("frame %d: cannot read a %dx%d image: %s\n", i, wI, hI, mdc_last_error());
+            return 1;
+        }
+        stack.insert(stack.end(), frame.begin(), frame.end());
+        exposures.push_back(mdc_seq_exposure(seq, i));
+        Hs.insert(Hs.end(), H, H + 9);
+    }
+    fclose(hf);
+    const int n = static_cast<int>(exposures.size());
+    printf("loaded %d images with a marker\n", n);
+    const size_t gwgh = static_cast<size_t>(opt.gw) * opt.gh;
+
+    // ---- front end on the device: gamma removal, normalisation + gradient invalidation, plane-to-image maps
+    CUDA_OR_DIE(cudaSetDevice(opt.device));
+    mdc_ctx* ctx = nullptr;
+    MDC_OR_DIE(mdc_ctx_create(opt.device, fov, photo, &ctx));
+    uint8_t* d_frames = nullptr;
+    float *d_images = nullptr, *d_p2x = nullptr, *d_p2y = nullptr, *d_plane = nullptr, *d_vig = nullptr, *d_smoothed = nullptr;
+    CUDA_OR_DIE(cudaMalloc(&d_images, npx * n * sizeof(float) + 4));
+    CUDA_OR_DIE(cudaMalloc(&d_p2x, gwgh * n * sizeof(float) + 4));
+    CUDA_OR_DIE(cudaMalloc(&d_p2y, gwgh * n * sizeof(float) + 4));
+    CUDA_OR_DIE(cudaMalloc(&d_plane, gwgh * sizeof(float)));
+    CUDA_OR_DIE(cudaMalloc(&d_vig, npx * sizeof(float)));
+    CUDA_OR_DIE(cudaMalloc(&d_smoothed, npx * sizeof(float)));
+    if (n > 0) {
+        CUDA_OR_DIE(cudaMalloc(&d_frames, stack.size()));
+        CUDA_OR_DIE(cudaMemcpy(d_frames, stack.data(), stack.size(), cudaMemcpyHostToDevice));
+        MDC_OR_DIE(mdc_unmap_u8(ctx, d_frames, d_images, static_cast<int>(npx), n, MDC_REMOVE_GAMMA, nullptr));      // getImage(i,false,true,false,false)
+        CUDA_OR_DIE(cudaFree(d_frames));
+        MDC_OR_DIE(mdc_vc_prepare_images(ctx, d_images, n, wI, hI, exposures.data(), mean_exposure, 255, d_images, nullptr));
+        MDC_OR_DIE(mdc_vc_plane_maps(fov, Hs.data(), n, opt.gw, opt.gh, opt.facw, opt.fach, d_p2x, d_p2y, opt.device, nullptr));
+    }
+
+    // ---- the optimisation loop: plane colour starts at 0 (the reference reads it uninitialised), vignette at 1 (:391)
+    CUDA_OR_DIE(cudaMemset(d_plane, 0, gwgh * sizeof(float)));
+    {
+        std::vector<float> ones(npx, 1.0f);
+        CUDA_OR_DIE(cudaMemcpy(d_vig, ones.data(), npx * sizeof(float), cudaMemcpyHostToDevice));
+    }
+    std::vector<double> log(static_cast<size_t>(4) * (opt.iterations > 0 ? opt.iterations : 1), 0.0);
+    MDC_OR_DIE(mdc_vignette_calib(ctx, d_images, d_p2x, d_p2y, n, opt.gw, opt.gh, wI, hI, opt.iterations, 15, 1, d_plane, d_vig, d_smoothed,
+                                  log.data()));
+
+    {
+        std::ofstream lf("vignetteCalibResult/log.txt", std::ios::trunc | std::ios::out);
+        lf.precision(15);
+        for (int it = 0; it < opt.iterations; ++it)
+            lf << it << " " << n << " " << log[4 * it + 3] << " " << sqrtf(static_cast<float>(log[4 * it + 2] / log[4 * it + 3])) << "\n";
+    }
+    int rc = 0;
+    if (opt.iterations > 0) {
+        std::vector<float> vig(npx), smoothed(npx), plane(gwgh);
+        CUDA_OR_DIE(cudaMemcpy(vig.data(), d_vig, npx * sizeof(float), cudaMemcpyDeviceToHost));
+        CUDA_OR_DIE(cudaMemcpy(smoothed.data(), d_smoothed, npx * sizeof(float), cudaMemcpyDeviceToHost));
+        CUDA_OR_DIE(cudaMemcpy(plane.data(), d_plane, gwgh * sizeof(float), cudaMemcpyDeviceToHost));
+        if (!write_plane_png("vignetteCalibResult/plane.png", plane, opt.gw, opt.gh) ||
+            !write_vignette_png("vignetteCalibResult/vignetteSmoothed.png", smoothed, wI, hI) ||
+            !write_vignette_png("vignetteCalibResult/vignette.png", vig, wI, hI)) {
+            printf("could not write the result images\n");
+            rc = 1;
+        }
+    }
+    cudaFree(d_images); cudaFree(d_p2x); cudaFree(d_p2y); cudaFree(d_plane); cudaFree(d_vig); cudaFree(d_smoothed);
+    mdc_ctx_destroy(ctx);
+    mdc_photo_destroy(photo);
+    mdc_fov_destroy(fov);
+    mdc_seq_close(seq);
+    return rc;
+}
