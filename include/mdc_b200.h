@@ -173,7 +173,9 @@ int mdc_undistort_f32(mdc_ctx* c, const float* d_in, float* d_out, int n_pix_in,
  *   d_frames      [n_frames][in_w*in_h] u8
  *   d_out_levels  array of `levels` device pointers; level l: [n_frames][w_l*h_l] f32.
  *                 Level 0 is the getImage result (out_w x out_h if MDC_RECTIFY else in_w x in_h).
- * levels = 1 gives exactly getImage.  This is the hot path (kernel K1). */
+ * levels = 1 gives exactly getImage.  This is the hot path (kernel K1).  One host thread may issue calls on one context to
+ * several streams at once; each staged K1 launch takes one of 64 work counters in turn, so at most 64 of them may be in flight
+ * per context. */
 int mdc_prepare_batch(mdc_ctx* c, const uint8_t* d_frames, int n_frames, unsigned flags,
                       float* const* d_out_levels, int levels, mdc_stream stream);
 /* Same with padded input rows: d_frames is [n_frames][in_h][row_pitch_bytes] (row_pitch_bytes >= in_w; rectifying mode only).
@@ -286,7 +288,9 @@ int mdc_estep(mdc_ctx* c, const uint8_t* d_data, int n, int npix, const double* 
  *   mdc_rc_rmse          out_host = {1e5*sqrt(mean((G[b]-t*E)^2 * 1e-10)), count}                       :50-69                         rounding-level
  *                        (the reference sums in long double); residuals, finite test and count exact; same bits on every run
  *   mdc_response_calib   the optimisation loop of main(): E := mean, then nits x {G-step, E-step, rescale}, rmse after
- *                        each half-step; log_host (may be NULL) receives nits x 4 doubles {rmse_G, rmse_E, rmse_rescaled, count}. */
+ *                        each half-step; log_host (may be NULL) receives nits x 4 doubles {rmse_G, rmse_E, rmse_rescaled, count}.
+ * These calls share scratch memory of the context (the leak-padding buffer, the G-step and rmse accumulators): do not run them on one
+ * context from several streams at once; give each stream its own context. */
 int mdc_rc_leak_padding(mdc_ctx* c, uint8_t* d_data, int n, int w, int h, int iterations, mdc_stream stream);
 int mdc_rc_einit(mdc_ctx* c, const uint8_t* d_data, int n, int npix, double* d_E, mdc_stream stream);
 int mdc_rc_gstep(mdc_ctx* c, const uint8_t* d_data, int n, int npix, const double* d_t, const double* d_E, double* d_G, mdc_stream stream);

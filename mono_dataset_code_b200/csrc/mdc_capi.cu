@@ -606,12 +606,14 @@ void tex_selfcheck(mdc_ctx* c) {
     float* la[1] = {out_a};
     float* lb[1] = {out_b};
     const long long launches0 = c->launches;
-    const int study0 = c->k1_study;
+    const int study0 = c->k1_study, use_tma0 = c->use_tma;
     c->k1_study = kStudyAll;             // the floor-study variants compute garbage by design
+    c->use_tma = -1;                     // MDC_USE_TMA=2/3 would refuse the texture loader while tex_ok is still false
     ok = ok && run_fused(c, frames, nf, u, la, 1, c->stream, 2, pitch) == MDC_OK;
     const bool tma_ref = tma_pitch_ok(c, frames, pitch);
     ok = ok && run_fused(c, frames, nf, u, lb, 1, c->stream, tma_ref ? 1 : 0, pitch) == MDC_OK;
     c->k1_study = study0;
+    c->use_tma = use_tma0;
     ok = ok && launch_count_mismatch(out_a, out_b, nf * n_out, d_bad, c->stream) == cudaSuccess;
     unsigned long long bad = ~0ull;
     ok = ok && cudaMemcpyAsync(&bad, d_bad, 8, cudaMemcpyDeviceToHost, c->stream) == cudaSuccess && cudaStreamSynchronize(c->stream) == cudaSuccess;

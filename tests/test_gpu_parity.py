@@ -63,7 +63,7 @@ def usable_loaders(prep):
 
 
 @pytest.mark.parametrize("name", list(CALIBS))
-@pytest.mark.parametrize("loader", ["tex", "tma", "ldg"])
+@pytest.mark.parametrize("loader", ["hybrid", "tex", "tma", "ldg"])
 def test_get_image_all_flag_combinations(name, loader, api, port, dataset_dir):
     iw, ih, ow, oh, mode, calib = CALIBS[name]
     files = dataset_dir(name, vignette_zeros=(name in ("odd_sizes", "c1_crop_640")))
