@@ -220,6 +220,7 @@ int mdc_seq_prepare(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned
  *   d_plane_color [gw*gh], d_vignette [wI*hI].  The marker detection and cv::findHomography stay with the caller; the maps and
  *   images come from mdc_vc_plane_maps and mdc_vc_prepare_images below.
  * Unlike the reference, which reads planeColor uninitialised in its first pass (:381, :425), the caller provides it.
+ * With n = 0, d_images, d_p2x and d_p2y may be null; the plane colour and the vignette then become NaN, as in the reference.
  * integer_abs: the reference's outlier test is `abs(residual) > oth2` on a double (:423, :481).  1 = the residual is truncated to
  *   int first, which is what that line does when only `int abs(int)` is visible to unqualified lookup (libstdc++ before GCC 6,
  *   i.e. the reference's era; also how the unmodified program builds against this repo's oracle headers); 0 = fabs(residual).
@@ -230,9 +231,10 @@ int mdc_seq_prepare(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned
 int mdc_vc_plane_step(mdc_ctx* c, const float* d_images, const float* d_p2x, const float* d_p2y, int n, int gw, int gh, int wI, int hI,
                       const float* d_vignette, float* d_plane_color, double outlier_th2, int integer_abs, double stats_host[2]);
 /* "optimize vignette" (:458-523) including the normalisation to maximum factor 1: d_vignette is read and overwritten.
- * The reference adds the scattered fp32 terms one after the other in fp32; here the same terms are added exactly (64-bit fixed
- * point), so the result differs from the reference by the rounding error of its own chain only (<= 2e-5 relative in the tests)
- * and is the same bits on every run. */
+ * The reference adds the scattered fp32 terms one after the other in fp32; here the same terms are rounded to a multiple of 2^-s
+ * (s from the largest colours and footprint count, DESIGN.md §4) and added exactly as 64-bit integers, so the result differs from
+ * the reference by the rounding error of its own chain and that rounding (<= 2e-5 relative in the tests) and is the same bits on
+ * every run.  Terms that are not finite are added in fp32, as the reference does. */
 int mdc_vc_vignette_step(mdc_ctx* c, const float* d_images, const float* d_p2x, const float* d_p2y, int n, int gw, int gh, int wI, int hI,
                          const float* d_plane_color, float* d_vignette, double outlier_th2, int integer_abs, double stats_host[2]);
 /* "dilate & smoothe" (:542-566): `iterations` rounds (the reference: 4) of the NaN-aware 3x3 mean.  Bit-identical. */

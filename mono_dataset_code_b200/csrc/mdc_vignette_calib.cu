@@ -175,8 +175,11 @@ __global__ void __launch_bounds__(256) vc_plane_kernel(const float* __restrict__
 // (one DADD with 1.5 * 2^52); the integers are added with 64-bit global REDs.  s comes from three numbers measured on the
 // device (VcFx): the largest finite |planeColor| and |image| bound every term, and the largest number of plane points whose
 // bilinear footprint starts at one pixel bounds how many terms a pixel can receive (4 x that), so that neither a term (< 2^50)
-// nor a sum (< 2^62) can overflow.  A term is thus off by at most 2^-50 of the largest possible term — far below one fp32 ulp of
-// any sum that passes the reference's TT >= 1 test — and the sums do not depend on the order of the atomics.
+// nor a sum (< 2^62) can overflow.  A term is off by at most 2^-(s+1), so a sum of K terms by at most K * 2^-(s+1), where
+// 2^-s <= max(2^-49, (4 * max_count + 4) * 2^-61) * 1.001 * P * max(P, I).  That is not always below one fp32 ulp of a sum that
+// passes the reference's TT >= 1 test: at 64 poses of 1000x1000 points in 1280x1024 images with values from 1 to 1e4 (max_count
+// 1679, s = 22) the largest error at TT >= 1 is 1.6 ulps (1.2e-7 relative), at TT >= 1e6 3e-13 relative.  The sums do not depend
+// on the order of the atomics.  tests/vc_fixed_point_spec.py states this arithmetic in numpy.
 struct VcFx { unsigned max_plane_bits, max_image_bits, max_count, pad; };
 constexpr double kVcMagic = 6755399441055744.0;      // 1.5 * 2^52
 __device__ __forceinline__ int vc_scale_exponent(const VcFx& fx) {
@@ -220,7 +223,11 @@ __global__ void __launch_bounds__(256) vc_umax_kernel(const unsigned* __restrict
     if ((threadIdx.x & 31) == 0 && m) atomicMax(out, m);
 }
 
-__device__ __forceinline__ void vc_add(long long* acc, float term, double scale) {
+// A finite term goes to the fixed-point sum.  One that is not - from an infinite colour, or a product of finite colours beyond
+// FLT_MAX, which the bounds do not cover - goes to the fp32 side sum, as the reference's fp32 chain would turn it into inf / NaN.
+// The side sums thus only ever hold +-inf or NaN, whose sum does not depend on the order of the atomics either.
+__device__ __forceinline__ void vc_add(long long* acc, float* special, float term, double scale) {
+    if (!isfinite(term)) { atomicAdd(special, term); return; }
     const double y = __dadd_rn(__dmul_rn(static_cast<double>(term), scale), kVcMagic);
     atomicAdd(reinterpret_cast<unsigned long long*>(acc), static_cast<unsigned long long>(__double_as_longlong(y) - __double_as_longlong(kVcMagic)));
 }
@@ -252,17 +259,12 @@ __global__ void __launch_bounds__(256) vc_vignette_kernel(const float* __restric
         const float a01 = __fmul_rn(__fmul_rn(t.w01, cP), cP), a11 = __fmul_rn(__fmul_rn(t.w11, cP), cP);
         const float b00 = __fmul_rn(__fmul_rn(t.w00, cI), cP), b10 = __fmul_rn(__fmul_rn(t.w10, cI), cP);
         const float b01 = __fmul_rn(__fmul_rn(t.w01, cI), cP), b11 = __fmul_rn(__fmul_rn(t.w11, cI), cP);
-        if (isfinite(cP) && isfinite(cI)) {
-            long long* a = tt + t.base;
-            long long* b = ct + t.base;
-            vc_add(a, a00, scale); vc_add(a + 1, a10, scale); vc_add(a + wI, a01, scale); vc_add(a + 1 + wI, a11, scale);
-            vc_add(b, b00, scale); vc_add(b + 1, b10, scale); vc_add(b + wI, b01, scale); vc_add(b + 1 + wI, b11, scale);
-        } else {                                                                           // an infinite colour: fp32 sums, which it turns into inf / NaN as in the reference
-            float* a = tt_special + t.base;
-            float* b = ct_special + t.base;
-            atomicAdd(a, a00); atomicAdd(a + 1, a10); atomicAdd(a + wI, a01); atomicAdd(a + 1 + wI, a11);
-            atomicAdd(b, b00); atomicAdd(b + 1, b10); atomicAdd(b + wI, b01); atomicAdd(b + 1 + wI, b11);
-        }
+        long long* a = tt + t.base;
+        long long* b = ct + t.base;
+        float* as = tt_special + t.base;
+        float* bs = ct_special + t.base;
+        vc_add(a, as, a00, scale); vc_add(a + 1, as + 1, a10, scale); vc_add(a + wI, as + wI, a01, scale); vc_add(a + 1 + wI, as + 1 + wI, a11, scale);
+        vc_add(b, bs, b00, scale); vc_add(b + 1, bs + 1, b10, scale); vc_add(b + wI, bs + wI, b01, scale); vc_add(b + 1 + wI, bs + 1 + wI, b11, scale);
         if (isnan(fac)) continue;
         e_sum += residual;
         r_cnt += 1.0;
@@ -409,7 +411,8 @@ unsigned vc_blocks(size_t work) {
 struct Problem { const float *images, *p2x, *p2y; int n, gwgh, wI, hI; };
 
 int check_problem(const char* who, mdc_ctx* c, const Problem& p, const void* a, const void* b) {
-    if (!c || !p.images || !p.p2x || !p.p2y || !a || !b || p.n < 0 || p.gwgh < 1 || p.wI < 2 || p.hI < 2) {
+    // with no images, nothing reads the images or the maps (an empty tensor's pointer may be null)
+    if (!c || (p.n > 0 && (!p.images || !p.p2x || !p.p2y)) || !a || !b || p.n < 0 || p.gwgh < 1 || p.wI < 2 || p.hI < 2) {
         mdc_set_error("%s: bad argument", who);
         return MDC_ERR_INVALID_ARG;
     }
