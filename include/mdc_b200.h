@@ -283,12 +283,17 @@ int mdc_estep(mdc_ctx* c, const uint8_t* d_data, int n, int npix, const double* 
  *   mdc_rc_einit         E = per-pixel mean over the n images                                          :249-259                       bit-exact
  *   mdc_rc_gstep         G[b] = sum(E[k]*t[i]) / count over samples with value b != 255, gaps extrapolated  :286-304   rounding-level: the products are
  *                        rounded as in the reference and then summed EXACTLY (fixed point), where the reference has one fp64 chain;
- *                        order-independent, so the same bits on every run and for every launch geometry.  (The fixed-point scale
- *                        comes from the largest finite |E| and |t|; if an exposure time is not finite, or that largest product
- *                        overflows, there is no common scale and the finite products are summed at unit resolution — garbage in.)
+ *                        order-independent, so the same bits on every run and for every launch geometry.  The fixed-point scale
+ *                        2^s comes from the exponents of the largest finite |E| and |t|, so every finite product keeps 48 bits
+ *                        below the largest one (and below 2^1024 when max|E| * max|t| overflows).  Non-finite products (an
+ *                        overflowing E*t, a NaN or infinite E or t) are summed in fp64 on the side and poison their bins as in
+ *                        the reference; a non-finite exposure time of a fully saturated frame changes nothing, as in the reference.
+ *                        With n = 0, d_data and d_t may be null (also for mdc_estep, mdc_rc_einit and mdc_rc_rmse).
  *   mdc_rc_rescale       factor = 255/G[255]; E *= factor; G *= factor; *factor_host = factor           :350-355                       bit-exact
  *   mdc_rc_rmse          out_host = {1e5*sqrt(mean((G[b]-t*E)^2 * 1e-10)), count}                       :50-69                         rounding-level
- *                        (the reference sums in long double); residuals, finite test and count exact; same bits on every run
+ *                        (the reference sums in long double); residuals, finite test and count exact; same bits on every run.
+ *                        The sums are fp64: where the sum of r^2 * 1e-10 passes 1.8e308 the result is inf, where the
+ *                        reference's long double would still be finite.
  *   mdc_response_calib   the optimisation loop of main(): E := mean, then nits x {G-step, E-step, rescale}, rmse after
  *                        each half-step; log_host (may be NULL) receives nits x 4 doubles {rmse_G, rmse_E, rmse_rescaled, count}.
  * These calls share scratch memory of the context (the leak-padding buffer, the G-step and rmse accumulators): do not run them on one

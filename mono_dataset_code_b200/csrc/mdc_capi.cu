@@ -956,7 +956,7 @@ void mdc_ctx_add_launches(mdc_ctx* c, int n) { c->launches += n; }
 void mdc_ctx_geometry(const mdc_ctx* c, int* in_w, int* in_h, int* out_w, int* out_h) { *in_w = c->in_w; *in_h = c->in_h; *out_w = c->out_w; *out_h = c->out_h; }
 
 extern "C" int mdc_estep(mdc_ctx* c, const uint8_t* d_data, int n, int npix, const double* d_t, const double* d_G, double* d_E, mdc_stream stream) {
-    if (!c || !d_data || !d_t || !d_G || !d_E || n < 0 || npix < 0) { mdc_set_error("mdc_estep: bad argument"); return MDC_ERR_INVALID_ARG; }
+    if (!c || (n > 0 && (!d_data || !d_t)) || !d_G || !d_E || n < 0 || npix < 0) { mdc_set_error("mdc_estep: bad argument"); return MDC_ERR_INVALID_ARG; }
     CU_CHECK(cudaSetDevice(c->device));
     cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
     CU_CHECK(launch_estep(d_data, n, npix, d_t, d_G, d_E, s));
@@ -985,7 +985,7 @@ extern "C" int mdc_rc_leak_padding(mdc_ctx* c, uint8_t* d_data, int n, int w, in
 }
 
 extern "C" int mdc_rc_einit(mdc_ctx* c, const uint8_t* d_data, int n, int npix, double* d_E, mdc_stream stream) {
-    if (!c || !d_data || !d_E || n < 0 || npix < 0) { mdc_set_error("mdc_rc_einit: bad argument"); return MDC_ERR_INVALID_ARG; }
+    if (!c || (n > 0 && !d_data) || !d_E || n < 0 || npix < 0) { mdc_set_error("mdc_rc_einit: bad argument"); return MDC_ERR_INVALID_ARG; }
     CU_CHECK(cudaSetDevice(c->device));
     cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
     if (npix > 0) { CU_CHECK(launch_rc_einit(d_data, n, npix, d_E, s)); c->launches++; }
@@ -996,7 +996,7 @@ extern "C" int mdc_rc_einit(mdc_ctx* c, const uint8_t* d_data, int n, int npix, 
 // the SAME images, so only the sums are accumulated
 static int rc_gstep_impl(mdc_ctx* c, const uint8_t* d_data, int n, int npix, const double* d_t, const double* d_E, double* d_G, bool reuse_counts,
                          mdc_stream stream) {
-    if (!c || !d_data || !d_t || !d_E || !d_G || n < 0 || npix < 0) { mdc_set_error("mdc_rc_gstep: bad argument"); return MDC_ERR_INVALID_ARG; }
+    if (!c || (n > 0 && (!d_data || !d_t)) || !d_E || !d_G || n < 0 || npix < 0) { mdc_set_error("mdc_rc_gstep: bad argument"); return MDC_ERR_INVALID_ARG; }
     CU_CHECK(cudaSetDevice(c->device));
     cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
     CU_CHECK(launch_rc_gstep(d_data, n, npix, d_t, d_E, c->d_rc, reinterpret_cast<unsigned long long*>(c->d_rc + 256), d_G, reuse_counts, c->d_rc + kRcFxOffset, s));
@@ -1093,7 +1093,7 @@ extern "C" int mdc_rc_rescale(mdc_ctx* c, int npix, double* d_E, double* d_G, do
 }
 
 extern "C" int mdc_rc_rmse(mdc_ctx* c, const uint8_t* d_data, int n, int npix, const double* d_t, const double* d_G, const double* d_E, double out_host[2]) {
-    if (!c || !d_data || !d_t || !d_G || !d_E || !out_host || n < 0 || npix < 0) { mdc_set_error("mdc_rc_rmse: bad argument"); return MDC_ERR_INVALID_ARG; }
+    if (!c || (n > 0 && (!d_data || !d_t)) || !d_G || !d_E || !out_host || n < 0 || npix < 0) { mdc_set_error("mdc_rc_rmse: bad argument"); return MDC_ERR_INVALID_ARG; }
     CU_CHECK(cudaSetDevice(c->device));
     CU_CHECK(launch_rc_rmse(d_data, n, npix, d_t, d_G, d_E, c->d_rc + 513, c->d_rc + 515, c->stream));
     c->launches += 2;

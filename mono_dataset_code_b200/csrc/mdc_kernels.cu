@@ -17,6 +17,7 @@
 // All of this is HBM-bound byte/float streaming; there is no GEMM-shaped work, so no tcgen05.
 #include <cuda.h>
 #include <cuda_runtime.h>
+#include <float.h>
 #include <stdint.h>
 #include <stdlib.h>
 
@@ -1359,7 +1360,8 @@ struct EstepOp {
 // largest finite |E| and |t| of the pass) such that every product is below 2^48 units; the conversion is one DADD with
 // 1.5 * 2^52 (round to nearest even), so a sample is off by at most 2^-48 of the largest product — the sum of 4 * 10^6 samples
 // of a bin is closer to the exact sum than the reference's own chain is.  Non-finite products (E = NaN of an all-saturated
-// pixel meeting t = 0 ...) go to a separate fp64 accumulator so that they poison G as they do in the reference.
+// pixel meeting t = 0, a NaN exposure time, a product that overflows ...) go to a separate fp64 accumulator so that they poison
+// G as they do in the reference; they do not change the scale, so every finite product keeps its 2^-48 resolution.
 //
 // Integer sums are also what makes the histogram cheap: shared memory has native 32-bit integer atomics (ATOMS.ADD, one
 // wavefront per conflict-free warp instruction) but only a compare-and-swap loop for 64-bit ones (LDS.64 + ATOMS.CAS.64, a
@@ -1373,16 +1375,23 @@ constexpr double kFxLimit = 281474976710656.0;       // 2^48: scaled products st
 // Four u64 words, so that the ranks of a pixel-sharded run can agree on one scale with a single all-reduce(MAX).
 struct GstepScale { unsigned long long max_e_bits, max_t_bits, bad_t, reserved; };
 
-// power of two 2^s with |E*t| * 2^s < 2^48 for all finite samples; kFxNoScale if no such bound exists (the largest product overflows
-// or an exposure time is not finite): every sample is then range-checked on its own
-constexpr int kFxNoScale = -100000;
+// s with |E*t| * 2^s < 2^48 for every FINITE product E*t of the pass: s = 47 - ilogb(max|E| * max|t|), the exponent of that product
+// taken from the two exponents and the product of the two mantissas, so that it exists where the product itself would overflow or
+// underflow.  A product that overflows is not finite and goes to the fp64 side sums; every finite one is below 2^1024, so s need not
+// go below 48 - 1024.  The range is wide (up to 47 + 2 * 1074), so 2^s is applied with scalbn, or as a multiply where it is a double.
+constexpr int kFxMinScale = 48 - 1024;
 __device__ __forceinline__ int gstep_scale_exponent(const GstepScale& sc) {
-    const double p = __dmul_rn(__longlong_as_double(static_cast<long long>(sc.max_e_bits)), __longlong_as_double(static_cast<long long>(sc.max_t_bits)));
-    if (!isfinite(p) || sc.bad_t) return kFxNoScale;
-    if (!(p > 0.0)) return 0;
-    int s = 48 - (ilogb(p) + 1);
-    return s < -1000 ? -1000 : (s > 1000 ? 1000 : s);
+    const double e = __longlong_as_double(static_cast<long long>(sc.max_e_bits)), t = __longlong_as_double(static_cast<long long>(sc.max_t_bits));
+    if (!(e > 0.0) || !(t > 0.0)) return 0;
+    const int ee = ilogb(e), et = ilogb(t);
+    const int s = 47 - (ee + et + ilogb(__dmul_rn(scalbn(e, -ee), scalbn(t, -et))));
+    return s < kFxMinScale ? kFxMinScale : s;
 }
+// The fast path forms (E * 2^s) * t, which is the reference's E * t times 2^s exactly when E * 2^s is exact (checked per lane) and
+// neither E * t nor the scaled product can leave the normal range in a way that changes an integer: for s in [-975, 1020] every
+// product is below 2^1023 and a product that underflows is worth less than 2^-2 units.  Outside that range, and in a pass with a
+// non-finite exposure time, every sample goes through the checked path.
+__device__ __forceinline__ bool gstep_fast_pass(const GstepScale& sc, int s) { return !sc.bad_t && s > kFxMinScale && s <= 1020; }
 // x (|x| < 2^48, already scaled) -> the integer nearest to it, as three limbs: value = l0 + l1 * 2^16 + l2 * 2^32, 0 <= l0, l1 < 2^16,
 // -2^16 <= l2 < 2^16.  bits(x + 1.5 * 2^52) = 0x4338000000000000 + value, so the limbs are bit fields of the sum.
 struct FxLimbs { uint32_t l0, l1; int l2; };
@@ -1437,20 +1446,22 @@ __device__ __forceinline__ void gstep_add(uint8_t* hist, uint32_t a, const FxLim
     atomicAdd(reinterpret_cast<int*>(p + 2 * kGstepPlaneBytes), v.l2);
     if (count) atomicAdd(reinterpret_cast<unsigned*>(p + 3 * kGstepPlaneBytes), 1u);
 }
-// one word with every sample range-checked (a non-finite E among the lane's pixels, or no usable scale); a free function with
-// everything passed by value so that the op's state stays in registers
+// one word with every sample range-checked (E * 2^s not exact for one of the lane's pixels, or no fast path in this pass): the
+// reference's product E * t, then scaled by 2^s; a free function with everything passed by value so that the op's state stays in
+// registers.  e0..e3 are the unscaled E.
 template <bool kCount>
-static __device__ __noinline__ void gstep_word_checked(uint8_t* hist, double* special, uint32_t lane8, double scale, uint32_t v, double ti,
+static __device__ __noinline__ void gstep_word_checked(uint8_t* hist, double* special, uint32_t lane8, int s, uint32_t v, double ti,
                                                        double e0, double e1, double e2, double e3) {
 #pragma unroll 1
     for (int j = 0; j < 4; ++j) {
         const uint32_t a = ((v >> (8 * j)) & 0xffu) << 8 | lane8;
         if (a >= 0xff00u) continue;      // saturated, :293
-        const double x = __dmul_rn(j == 0 ? e0 : (j == 1 ? e1 : (j == 2 ? e2 : e3)), ti);
+        const double p = __dmul_rn(j == 0 ? e0 : (j == 1 ? e1 : (j == 2 ? e2 : e3)), ti);      // :295
+        const double x = scalbn(p, s);   // exact, or (below 2^-1022) worth nothing after rounding to an integer
         if (fx_in_range(x)) {
             gstep_add(hist, a, fx_limbs(x), kCount);
-        } else {
-            atomicAdd(special + (a >> 8), __ddiv_rn(x, scale));
+        } else {                         // only a non-finite product
+            atomicAdd(special + (a >> 8), p);
             if (kCount) atomicAdd(reinterpret_cast<unsigned*>(hist + (a >> 1) + 3 * kGstepPlaneBytes), 1u);
         }
     }
@@ -1473,23 +1484,28 @@ struct GstepOp {
     int groups_since_fold;
     const double* E;
     double* special;
-    double scale;                     // 2^s
-    double e[4];
-    uint32_t mode;                    // 0: fast path; 1: every sample range-checked (a non-finite E among this lane's pixels, or no usable scale); 2: no pixels
-    bool no_scale;
+    double scale;                     // 2^s, or 0 if this pass has no fast path (gstep_fast_pass)
+    double e[4];                      // E * 2^s (fast path) or E (checked path)
+    uint32_t mode;                    // 0: fast path; 1: every sample range-checked (E * 2^s not exact for one of this lane's pixels, or no fast path); 2: no pixels
+    int s;
     __device__ __forceinline__ GstepOp(uint8_t* region, const Params& p)
         : hist(region), lane8((threadIdx.x & 31) * 8u), groups_since_fold(0), E(p.E), special(p.fx.special), mode(2u) {
-        const int s = gstep_scale_exponent(*p.fx.scale);
-        no_scale = s == kFxNoScale;
-        scale = no_scale ? 1.0 : scalbn(1.0, s);
+        s = gstep_scale_exponent(*p.fx.scale);
+        scale = gstep_fast_pass(*p.fx.scale, s) ? scalbn(1.0, s) : 0.0;
     }
     __device__ __forceinline__ void begin_tile(size_t k0, bool act) {
-        mode = !act ? 2u : (no_scale ? 1u : 0u);
+        mode = !act ? 2u : (scale == 0.0 ? 1u : 0u);
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const double ek = act ? E[k0 + j] : 0.0;
-            if (!isfinite(ek)) mode |= 1u;
-            e[j] = __dmul_rn(ek, scale);      // exact: (E * 2^s) * t == (E * t) * 2^s
+            const double sk = __dmul_rn(ek, scale);
+            // exact unless it overflowed (or E is not finite) or lost bits below 2^-1022; then (E * 2^s) * t != (E * t) * 2^s
+            if (!(fabs(sk) <= DBL_MAX) || (fabs(sk) < DBL_MIN && ek != 0.0)) mode |= 1u;
+            e[j] = sk;
+        }
+        if (mode == 1u) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) e[j] = E[k0 + j];
         }
     }
     // a: (value << 8) | lane * 8, i.e. twice the byte offset of this lane's slot in a plane.  Saturated samples (:293) are not skipped:
@@ -1497,7 +1513,7 @@ struct GstepOp {
     __device__ __forceinline__ void add(uint32_t a, const FxLimbs& v) { gstep_add(hist, a, v, kCount); }
     __device__ __forceinline__ void word(uint32_t v, double ti) {
         if (mode) {
-            if (mode == 1u) gstep_word_checked<kCount>(hist, special, lane8, scale, v, ti, e[0], e[1], e[2], e[3]);
+            if (mode == 1u) gstep_word_checked<kCount>(hist, special, lane8, s, v, ti, e[0], e[1], e[2], e[3]);
             return;
         }
         add(__byte_perm(v, lane8, 0x5504), fx_limbs(__dmul_rn(e[0], ti)));
@@ -1543,8 +1559,11 @@ struct GstepOp {
 // The reference keeps e in a long double, so its bits are out of reach anyway; what is kept exact is every residual r (one DMUL,
 // one DADD, as the reference rounds it), the finite test on it and the count.  The squares of a word's four samples are summed
 // with DFMA (saturated ones predicated off) and the factor 1e-10 is applied once at the end; a word whose partial sum is not finite
-// — some r is NaN / inf, or a square overflowed — is redone sample by sample in the reference's own form (r*r*1e-10).  Five
-// instructions per sample instead of twelve; saturated samples are predicated off.
+// — some r is NaN / inf, or a square overflowed — or is 2^900 or more is redone sample by sample in the reference's own form
+// (r*r*1e-10).  The bound keeps the unscaled sum finite over up to 2^34 words per thread (2^934 < 2^1024), so squares of residuals
+// near 1e153, each finite, cannot add up to inf where the reference's scaled sum does not.  Five instructions per sample instead of
+// twelve; saturated samples are predicated off.
+constexpr uint32_t kRmseFastBelow = 0x78300000u;      // high word of 2^900 (biased exponent 1023 + 900)
 struct RmseChecked { double err; unsigned dropped; };
 // one word, sample by sample, in the reference's own form; a free function with everything passed by value so that the op's state
 // stays in registers
@@ -1603,7 +1622,7 @@ struct RmseOp {
         double w01 = 0.0, w23 = 0.0;
         square(a0, r0, w01); square(a2, r2, w23); square(a1, r1, w01); square(a3, r3, w23);
         const double w = w01 + w23;
-        if ((static_cast<uint32_t>(__double2hiint(w)) & 0x7ff00000u) != 0x7ff00000u) {      // finite: four finite residuals (or saturated samples)
+        if ((static_cast<uint32_t>(__double2hiint(w)) & 0x7ff00000u) < kRmseFastBelow) {      // finite and below 2^900: four finite residuals (or saturated samples)
             sq += w;
         } else {
             const RmseChecked c = rmse_word_checked(table, lane8, v, ti, e[0], e[1], e[2], e[3]);
@@ -1673,7 +1692,7 @@ static cudaError_t launch_stream(const StreamArgs& a, const typename Op::Params&
     if (grid_out) *grid_out = static_cast<int>(grid);
     // exposure times -> constant memory (device-to-device, on this stream), behind the last pass that read the symbol
     cudaEvent_t* last_reader = g_exposure_reader;      // one event per device, shared by the three ops (they share the symbol)
-    const bool use_const = a.n <= kEbMaxN && dev >= 0 && dev < 64;
+    const bool use_const = a.n > 0 && a.n <= kEbMaxN && dev >= 0 && dev < 64;      // (no frames: nothing to copy, t may be null)
     if (use_const) {
         if (!last_reader[dev] && (e = cudaEventCreateWithFlags(&last_reader[dev], cudaEventDisableTiming)) != cudaSuccess) return e;
         else if ((e = cudaStreamWaitEvent(stream, last_reader[dev], 0)) != cudaSuccess) return e;
@@ -1783,16 +1802,18 @@ __global__ void __launch_bounds__(256) rc_gstep_accum_kernel(const uint8_t* __re
     s_lo[threadIdx.x] = 0ull; s_hi[threadIdx.x] = 0; s_num[threadIdx.x] = 0ull;
     __syncthreads();
     const int se = gstep_scale_exponent(*fx.scale);
-    const double scale = se == kFxNoScale ? 1.0 : scalbn(1.0, se);
+    const bool mul = se >= -1022 && se <= 1023;      // 2^s is a double: p * 2^s and scalbn(p, s) are the same correctly rounded value
+    const double scale = mul ? scalbn(1.0, se) : 1.0;
     const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
     for (size_t k = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; k < npix; k += stride) {
-        const double e = __dmul_rn(E[k], scale);
+        const double e = E[k];
         for (int i = 0; i < n; ++i) {
             const unsigned b = data[static_cast<size_t>(i) * npix + k];
             if (b == 255u) continue;
             atomicAdd(&s_num[b], 1ull);
-            const double x = __dmul_rn(e, __ldg(t + i));
-            if (!fx_in_range(x)) { atomicAdd(fx.special + b, __ddiv_rn(x, scale)); continue; }
+            const double p = __dmul_rn(e, __ldg(t + i));      // :295
+            const double x = mul ? __dmul_rn(p, scale) : scalbn(p, se);
+            if (!fx_in_range(x)) { atomicAdd(fx.special + b, p); continue; }      // only a non-finite product
             const long long v = __double_as_longlong(__dadd_rn(x, kFxMagic)) - __double_as_longlong(kFxMagic);
             const unsigned long long uv = static_cast<unsigned long long>(v);
             const unsigned long long old = atomicAdd(&s_lo[b], uv);
@@ -1808,8 +1829,7 @@ __global__ void __launch_bounds__(256) rc_gstep_accum_kernel(const uint8_t* __re
 
 // gsum[b] = (hi * 2^64 + lo) * 2^-s + special[b]: the 128-bit sums back in fp64 (two roundings at most, the same on every run)
 __device__ __forceinline__ double fx_to_double(unsigned long long lo, unsigned long long hi, const GstepScale& scale, double special) {
-    int s = gstep_scale_exponent(scale);
-    if (s == kFxNoScale) s = 0;
+    const int s = gstep_scale_exponent(scale);
     const double h = __dmul_rn(static_cast<double>(static_cast<long long>(hi)), 18446744073709551616.0);
     return __dadd_rn(scalbn(__dadd_rn(h, static_cast<double>(lo)), -s), special);
 }
