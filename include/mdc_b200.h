@@ -123,7 +123,13 @@ int mdc_ctx_create(int device, const mdc_fov* fov, const mdc_photo* photo, mdc_c
  * (the host language's NCCL binding, e.g. torch.distributed) into DEVICE buffers the
  * caller owns, and every rank adopts them here.  Pointers may be NULL for a missing
  * half (d_remap_* NULL = no rectifier; d_ginv / d_vinv NULL = not loaded).  The buffers
- * must outlive the context. */
+ * must outlive the context.
+ * Every remap entry (x, y) must lie where undistort reads inside the frame (FOVUndistorter.cpp:347-365):
+ *   x < 0 (a black pixel; y may then be anything, NaN included), or
+ *   0 <= x < in_w-1 and -1 < y < in_h-1, both finite (-0.0 counts as 0; a y in (-1, 0) truncates to row 0).
+ * The tables UndistorterFOV builds always do.  Any other entry (x = in_w-1, y = in_h-1, y = -1, a NaN or infinite x, a NaN y
+ * under a valid x) makes the call fail with MDC_ERR_INVALID_ARG before any kernel runs; mdc_last_error() names the first such
+ * output pixel and its values.  The check reads the host copy of the tables that the tile plan is built from. */
 int mdc_ctx_create_from_device_tables(int device, int in_w, int in_h, int out_w, int out_h,
                                       const float* d_remap_x, const float* d_remap_y,
                                       const float* d_ginv256, const float* d_vinv, mdc_ctx** out);

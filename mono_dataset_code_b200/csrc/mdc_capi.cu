@@ -117,9 +117,28 @@ int ensure_bytes(void** p, size_t* have, size_t need) {
     return MDC_OK;
 }
 
-// Build the tile plan from HOST copies of the remap tables.
+// Every entry of the remap tables must lie in the domain inside which the reference's undistort reads only pixels of the frame
+// (FOVUndistorter.cpp:347-365): x < 0 (black, whatever y holds), or 0 <= x < in_w-1 and -1 < y < in_h-1 (truncation toward zero
+// makes the row of a y in (-1, 0) row 0).  NaN and infinite coordinates are outside it, except a y under a negative x.  The tile
+// plan and the kernels rely on this: a box, tap or vignette index is never clamped.
+int check_table_domain(const float* rx, const float* ry, int out_w, int out_h, int in_w, int in_h) {
+    const size_t n = static_cast<size_t>(out_w) * out_h;
+    for (size_t i = 0; i < n; ++i) {
+        const float x = rx[i], y = ry[i];
+        if (x < 0) continue;
+        // compared in double: in_w-1 and in_h-1 are not always floats
+        if (static_cast<double>(x) < in_w - 1.0 && static_cast<double>(y) > -1.0 && static_cast<double>(y) < in_h - 1.0) continue;
+        mdc_set_error("remap table entry at output pixel (%zu, %zu) is (x %.9g, y %.9g): outside the domain x < 0, or 0 <= x < %d and -1 < y < %d, "
+                      "in which undistort reads inside the %d x %d input frame", i % static_cast<size_t>(out_w), i / static_cast<size_t>(out_w),
+                      static_cast<double>(x), static_cast<double>(y), in_w - 1, in_h - 1, in_w, in_h);
+        return MDC_ERR_INVALID_ARG;
+    }
+    return MDC_OK;
+}
+
+// Build the tile plan from HOST copies of the remap tables (inside the domain of check_table_domain).
 void build_plan(mdc_ctx* c, const float* rx, const float* ry) {
-    const int OW = c->out_w, OH = c->out_h, W = c->in_w, H = c->in_h;
+    const int OW = c->out_w, OH = c->out_h;
     c->tiles_x = (OW + kTile - 1) / kTile;
     c->tiles_y = (OH + kTile - 1) / kTile;
     const int n_tiles = c->tiles_x * c->tiles_y;
@@ -148,9 +167,6 @@ void build_plan(mdc_ctx* c, const float* rx, const float* ry) {
             }
         TileDesc td{0, 0, 0, TILE_EMPTY};
         if (xhi >= 0) {
-            // defensive: a table that violates the reference's in-bounds guarantee would read outside the frame
-            xlo = std::max(xlo, 0); ylo = std::max(ylo, 0);
-            xhi = std::min(xhi, W - 1); yhi = std::min(yhi, H - 1);
             const int x0 = tma_geom_ok ? (xlo & ~15) : (xlo & ~3);   // TMA faults on box origins that are not 16-byte aligned
             const int bh = yhi - ylo + 1, bh8 = (bh + gran - 1) / gran * gran;
             // Box width = shared-memory pitch of the staged box.  The tap loads of a warp (32 lanes = one output
@@ -222,15 +238,21 @@ void build_plan(mdc_ctx* c, const float* rx, const float* ry) {
         c->tiles[t] = td;
     }
     if (getenv("MDC_VERBOSE")) {
-        long staged_bytes = 0; int n_staged = 0;
-        for (const TileDesc& t : c->tiles) if ((t.mode_map & 0x0f) == TILE_STAGED) { staged_bytes += (t.bw_bh & 0xffff) * (t.mode_map >> 16); ++n_staged; }
-        fprintf(stderr, "[mdc] plan: %d tiles (%d staged), %zu TMA box classes at row granularity %d, largest box %d B, mean box %ld B\n",
-                n_tiles, n_staged, c->classes.size(), gran, c->box_px_max, n_staged ? staged_bytes / n_staged : 0);
+        long staged_bytes = 0; int n_staged = 0, n_direct = 0, n_empty = 0, n_black = 0;
+        for (const TileDesc& t : c->tiles) {
+            const int mode = t.mode_map & 0x0f;
+            if (mode == TILE_STAGED) { staged_bytes += (t.bw_bh & 0xffff) * (t.mode_map >> 16); ++n_staged; }
+            n_direct += mode == TILE_DIRECT;
+            n_empty += mode == TILE_EMPTY;
+            n_black += (t.mode_map & TILE_HAS_BLACK) != 0;
+        }
+        fprintf(stderr, "[mdc] plan: %d tiles (%d staged, %d direct, %d empty, %d with black pixels), %zu TMA box classes at row granularity %d, "
+                "largest box %d B, mean box %ld B\n", n_tiles, n_staged, n_direct, n_empty, n_black, c->classes.size(), gran, c->box_px_max,
+                n_staged ? staged_bytes / n_staged : 0);
     }
     if (static_cast<int>(c->classes.size()) <= kMaxClasses) break;
     }
     c->plan_tma_ok = !c->classes.empty() && static_cast<int>(c->classes.size()) <= kMaxClasses && encode_tiled_fn() != nullptr;
-    (void)W; (void)H;
 }
 
 int upload_plan(mdc_ctx* c) {
@@ -709,6 +731,7 @@ extern "C" int mdc_ctx_create_from_device_tables(int device, int in_w, int in_h,
         cudaError_t e = cudaMemcpy(hx.data(), d_remap_x, n * sizeof(float), cudaMemcpyDeviceToHost);
         if (e == cudaSuccess) e = cudaMemcpy(hy.data(), d_remap_y, n * sizeof(float), cudaMemcpyDeviceToHost);
         if (e != cudaSuccess) { mdc_set_error("reading back remap tables failed: %s", cudaGetErrorString(e)); mdc_ctx_destroy(c); return MDC_ERR_CUDA; }
+        if ((rc = check_table_domain(hx.data(), hy.data(), out_w, out_h, in_w, in_h)) != MDC_OK) { mdc_ctx_destroy(c); return rc; }
         build_plan(c, hx.data(), hy.data());
         if ((rc = upload_plan(c)) != MDC_OK) { mdc_ctx_destroy(c); return rc; }
     }
