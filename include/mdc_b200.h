@@ -157,6 +157,11 @@ int mdc_ctx_configure(mdc_ctx* c, int use_tma, int ctas_per_sm);
 int mdc_ctx_loader_usable(const mdc_ctx* c, int loader);
 /* The MDC_LOADER_* that use_tma = -1 resolves to for this context. */
 int mdc_ctx_auto_loader(const mdc_ctx* c);
+/* The same two answers for frames whose rows are row_pitch_bytes apart (mdc_prepare_batch_pitched, and the padded rows that
+ * mdc_prepare_batch_host copies to the device); the two calls above answer for tightly packed rows (row_pitch_bytes = in_w).
+ * A pitch below in_w or above 2^30 is usable by no loader (and resolves to MDC_LOADER_LDG). */
+int mdc_ctx_loader_usable_pitched(const mdc_ctx* c, int loader, size_t row_pitch_bytes);
+int mdc_ctx_auto_loader_pitched(const mdc_ctx* c, size_t row_pitch_bytes);
 
 /* -------------------------------------------------------------------------------------
  * Device-resident per-frame operators (all pointers are DEVICE pointers; `stream` is a
@@ -186,7 +191,8 @@ int mdc_prepare_batch(mdc_ctx* c, const uint8_t* d_frames, int n_frames, unsigne
                       float* const* d_out_levels, int levels, mdc_stream stream);
 /* Same with padded input rows: d_frames is [n_frames][in_h][row_pitch_bytes] (row_pitch_bytes >= in_w; rectifying mode only).
  * A pitch that is a multiple of 16 bytes keeps image widths that are NOT a multiple of 16 on the TMA loader (a tightly packed odd
- * width can only use the ~2x slower LDG loader); mdc_prepare_batch_host pads such rows itself during its host-to-device copy. */
+ * width can only use the ~2x slower LDG loader); mdc_prepare_batch_host pads such rows itself during its host-to-device copy, in
+ * rectifying mode, to the next multiple of 32 bytes (when the context's tile plan can use TMA at all). */
 int mdc_prepare_batch_pitched(mdc_ctx* c, const uint8_t* d_frames, size_t row_pitch_bytes, int n_frames, unsigned flags,
                               float* const* d_out_levels, int levels, mdc_stream stream);
 
@@ -214,9 +220,11 @@ float mdc_seq_exposure(const mdc_seq* s, int id);         /* getExposure(), :179
  * out may be NULL to query the size only.  MDC_ERR_FORMAT if the frame cannot be decoded. */
 int mdc_seq_read_gray8(const mdc_seq* s, int id, uint8_t* out, size_t capacity, int* w, int* h);
 /* getImage(id, flags...) for id in [first, first+count) into HOST level buffers (level l: [count][(w>>l)*(h>>l)] floats, as for
- * mdc_prepare_batch_host): `threads` host threads (0 = all) decode the next chunk (one frame per thread, 32..256 frames) into pinned
- * memory while the current chunk goes through H2D -> fused kernel -> D2H.  A frame of the wrong size or an undecodable one stops the call with MDC_ERR_FORMAT
- * (the reference prints and returns 0 for that frame, :194-205). */
+ * mdc_prepare_batch_host): `threads` host threads (0 = all) decode the next chunk (two frames per decode thread, 16..256 frames) into
+ * pinned memory while the current chunk goes through H2D -> fused kernel -> D2H.  A frame of the wrong size or an undecodable one stops the call with MDC_ERR_FORMAT
+ * (the reference prints and returns 0 for that frame, :194-205); the chunks before the one holding that frame are complete, the
+ * rows from that chunk on are not written.  first / count outside the sequence, levels outside 1..MDC_MAX_PYR_LEVELS or a NULL
+ * level that has pixels (a level without pixels may be NULL) return MDC_ERR_INVALID_ARG before anything is decoded. */
 int mdc_seq_prepare(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned flags, float* const* h_out_levels, int levels, int threads);
 
 /* =====================================================================================
@@ -346,8 +354,9 @@ int mdc_rc_gstep_finish_exact(mdc_ctx* c, const unsigned long long* d_scale4, co
 int mdc_unmap_u8_host(mdc_ctx* c, const uint8_t* in, float* out, int n, unsigned flags);
 int mdc_undistort_u8_host(mdc_ctx* c, const uint8_t* in, float* out, int n_pix_in, int n_pix_out);
 int mdc_undistort_f32_host(mdc_ctx* c, const float* in, float* out, int n_pix_in, int n_pix_out);
-/* getImage for n_frames host frames; out_levels[l] host buffers laid out as in mdc_prepare_batch.
- * Internally chunked and double-buffered so H2D, kernel and D2H overlap. */
+/* getImage for n_frames host frames; out_levels[l] host buffers laid out as in mdc_prepare_batch (NULL only for a level without
+ * pixels).  Internally chunked (MDC_HOST_CHUNK frames, default 16) on three streams so H2D, kernel and D2H overlap; returns
+ * after the last copy into out_levels has landed. */
 int mdc_prepare_batch_host(mdc_ctx* c, const uint8_t* frames, int n_frames, unsigned flags,
                            float* const* out_levels, int levels);
 /* Pinned host memory for the calling thread's current CUDA device, placed on the NUMA node that device is attached to

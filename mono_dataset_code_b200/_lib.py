@@ -73,6 +73,8 @@ SIGNATURES = {
     "mdc_ctx_configure": (C.c_int, [_vp, C.c_int, C.c_int]),
     "mdc_ctx_loader_usable": (C.c_int, [_vp, C.c_int]),
     "mdc_ctx_auto_loader": (C.c_int, [_vp]),
+    "mdc_ctx_loader_usable_pitched": (C.c_int, [_vp, C.c_int, C.c_size_t]),
+    "mdc_ctx_auto_loader_pitched": (C.c_int, [_vp, C.c_size_t]),
     "mdc_unmap_u8": (C.c_int, [_vp, _vp, _vp, C.c_int, C.c_int, C.c_uint, _vp]),
     "mdc_undistort_u8": (C.c_int, [_vp, _vp, _vp, C.c_int, C.c_int, C.c_int, _vp]),
     "mdc_undistort_f32": (C.c_int, [_vp, _vp, _vp, C.c_int, C.c_int, C.c_int, _vp]),

@@ -262,14 +262,18 @@ class Context:
             use_tma = self.LOADERS[use_tma]
         check(lib.mdc_ctx_configure(self._h, use_tma, ctas_per_sm), "mdc_ctx_configure")
 
-    def auto_loader(self) -> str:
-        i = int(lib.mdc_ctx_auto_loader(self._h))
+    def auto_loader(self, row_pitch: int | None = None) -> str:
+        """The loader use_tma = -1 resolves to, for tightly packed rows or rows `row_pitch` bytes apart."""
+        i = int(lib.mdc_ctx_auto_loader(self._h) if row_pitch is None else lib.mdc_ctx_auto_loader_pitched(self._h, row_pitch))
         return [k for k, v in self.LOADERS.items() if v == i][0]
 
-    def loader_usable(self, loader) -> bool:
+    def loader_usable(self, loader, row_pitch: int | None = None) -> bool:
+        """Whether `loader` can run on this context's frames: tightly packed rows, or rows `row_pitch` bytes apart."""
         if isinstance(loader, str):
             loader = self.LOADERS[loader]
-        return bool(lib.mdc_ctx_loader_usable(self._h, loader))
+        if row_pitch is None:
+            return bool(lib.mdc_ctx_loader_usable(self._h, loader))
+        return bool(lib.mdc_ctx_loader_usable_pitched(self._h, loader, row_pitch))
 
     @property
     def launch_count(self) -> int:

@@ -790,17 +790,28 @@ extern "C" int mdc_ctx_configure(mdc_ctx* c, int use_tma, int ctas_per_sm) {
     return MDC_OK;
 }
 
-extern "C" int mdc_ctx_auto_loader(const mdc_ctx* c) { return c && c->have_fov ? auto_loader(c, nullptr, c->in_w) : 0; }
+static bool pitch_valid(const mdc_ctx* c, size_t row_pitch_bytes) {
+    return c && c->have_fov && row_pitch_bytes >= static_cast<size_t>(c->in_w) && row_pitch_bytes <= (1u << 30);
+}
 
-extern "C" int mdc_ctx_loader_usable(const mdc_ctx* c, int loader) {
-    if (!c || !c->have_fov) return 0;
+extern "C" int mdc_ctx_auto_loader_pitched(const mdc_ctx* c, size_t row_pitch_bytes) {
+    return pitch_valid(c, row_pitch_bytes) ? auto_loader(c, nullptr, static_cast<int>(row_pitch_bytes)) : 0;
+}
+extern "C" int mdc_ctx_auto_loader(const mdc_ctx* c) { return c ? mdc_ctx_auto_loader_pitched(c, static_cast<size_t>(c->in_w)) : 0; }
+
+extern "C" int mdc_ctx_loader_usable_pitched(const mdc_ctx* c, int loader, size_t row_pitch_bytes) {
+    if (!pitch_valid(c, row_pitch_bytes)) return 0;
+    const int pitch = static_cast<int>(row_pitch_bytes);
     switch (loader) {
         case MDC_LOADER_LDG: return 1;
-        case MDC_LOADER_TMA: return tma_pitch_ok(c, nullptr, c->in_w) ? 1 : 0;      // for tightly packed frames
-        case MDC_LOADER_TEX: return (c->tex_ok && c->in_w % c->tex_pitch_align == 0) ? 1 : 0;      // for tightly packed frames
-        case MDC_LOADER_HYBRID: return (c->tex_ok && c->in_w % c->tex_pitch_align == 0 && tma_pitch_ok(c, nullptr, c->in_w)) ? 1 : 0;
+        case MDC_LOADER_TMA: return tma_pitch_ok(c, nullptr, pitch) ? 1 : 0;
+        case MDC_LOADER_TEX: return (c->tex_ok && pitch % c->tex_pitch_align == 0) ? 1 : 0;
+        case MDC_LOADER_HYBRID: return (c->tex_ok && pitch % c->tex_pitch_align == 0 && tma_pitch_ok(c, nullptr, pitch)) ? 1 : 0;
         default: return 0;
     }
+}
+extern "C" int mdc_ctx_loader_usable(const mdc_ctx* c, int loader) {      // for tightly packed frames
+    return c ? mdc_ctx_loader_usable_pitched(c, loader, static_cast<size_t>(c->in_w)) : 0;
 }
 
 // --------------------------------------------------------------- device-resident operators
@@ -1245,13 +1256,18 @@ extern "C" int mdc_prepare_batch_host(mdc_ctx* c, const uint8_t* frames, int n_f
     }
     if (c->in_w < 1) { mdc_set_error("mdc_prepare_batch_host: context has no image geometry"); return MDC_ERR_INVALID_OBJECT; }
     const bool rectify = (flags & MDC_RECTIFY) != 0;
+    const int w0 = rectify ? c->out_w : c->in_w, h0 = rectify ? c->out_h : c->in_h;
+    size_t lvl_px[MDC_MAX_PYR_LEVELS], px_per_frame = 0;
+    for (int l = 0; l < levels; ++l) {
+        lvl_px[l] = static_cast<size_t>(w0 >> l) * (h0 >> l);
+        px_per_frame += lvl_px[l];
+        // checked before any copy: a NULL host level that has pixels would otherwise reach cudaMemcpyAsync after earlier chunks ran
+        if (!out_levels[l] && lvl_px[l] > 0) { mdc_set_error("mdc_prepare_batch_host: output level %d is NULL", l); return MDC_ERR_INVALID_ARG; }
+    }
     if (rectify && !c->have_fov) { mdc_set_error("getImage(rectify) on an invalid rectifier"); return MDC_ERR_INVALID_OBJECT; }
     if (n_frames == 0) return MDC_OK;
     CU_CHECK(cudaSetDevice(c->device));
     const size_t n_in = static_cast<size_t>(c->in_w) * c->in_h;
-    const int w0 = rectify ? c->out_w : c->in_w, h0 = rectify ? c->out_h : c->in_h;
-    size_t lvl_px[MDC_MAX_PYR_LEVELS], px_per_frame = 0;
-    for (int l = 0; l < levels; ++l) { lvl_px[l] = static_cast<size_t>(w0 >> l) * (h0 >> l); px_per_frame += lvl_px[l]; }
     // chunking: enough frames per kernel to fill the machine, small enough to overlap copy and compute
     const char* e = getenv("MDC_HOST_CHUNK");
     int chunk = e ? atoi(e) : 16;

@@ -4,7 +4,7 @@
 //   mdc_seq_open      images/ folder (sorted) or, if that is empty, images.zip (central directory, sorted names); times.txt
 //   mdc_seq_read_gray8 getImageRaw_internal with CV_LOAD_IMAGE_GRAYSCALE: 8/16-bit grey PNG (16 -> 8 bit by dropping the low byte, as
 //                     OpenCV's reader does), binary PGM, baseline JPEG (mdc_jpeg.cpp) - the same bytes as cv::imread returns.
-//   mdc_seq_prepare   getImage for a range of frames: worker threads decode chunk k+1 (32..256 frames, one per thread) into
+//   mdc_seq_prepare   getImage for a range of frames: worker threads decode chunk k+1 (two frames per thread, 16..256 frames) into
 //                     pinned memory while chunk k goes through mdc_prepare_batch_host (H2D, fused kernel, D2H on three streams).
 //
 // The zip reader handles what `zip` / Python's zipfile / the TUM archives produce: stored and deflated entries, no encryption,
@@ -290,19 +290,33 @@ static int default_decode_threads() {
 // getImage(id, ...) for ids [first, first+count): decode ahead on `threads` host threads, prepare on the GPU chunk by chunk.
 extern "C" int mdc_seq_prepare(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned flags, float* const* h_out_levels, int levels,
                                int threads) {
-    if (!c || !s || first < 0 || count < 0 || first + count > static_cast<int>(s->files.size()) || !h_out_levels || levels < 1) {
-        mdc_set_error("mdc_seq_prepare: bad argument");
+    // Everything that does not depend on the context is checked first, and all of it before any staging or thread work.  The range
+    // test is written so that it cannot overflow (first + count can).
+    if (!s || !h_out_levels) { mdc_set_error("mdc_seq_prepare: bad argument"); return MDC_ERR_INVALID_ARG; }
+    const int n_files = static_cast<int>(s->files.size());
+    if (first < 0 || count < 0 || first > n_files || count > n_files - first) {
+        mdc_set_error("mdc_seq_prepare: frames first = %d, count = %d outside the sequence's %d", first, count, n_files);
         return MDC_ERR_INVALID_ARG;
     }
-    if (count == 0) return MDC_OK;
+    if (levels < 1 || levels > MDC_MAX_PYR_LEVELS) {
+        mdc_set_error("mdc_seq_prepare: %d pyramid levels (1..%d)", levels, MDC_MAX_PYR_LEVELS);
+        return MDC_ERR_INVALID_ARG;
+    }
+    if (!c) { mdc_set_error("mdc_seq_prepare: bad argument"); return MDC_ERR_INVALID_ARG; }
     int in_w = 0, in_h = 0, out_w = 0, out_h = 0;
     mdc_ctx_geometry(c, &in_w, &in_h, &out_w, &out_h);
     if (in_w < 1 || in_h < 1) { mdc_set_error("mdc_seq_prepare: context has no image geometry"); return MDC_ERR_INVALID_OBJECT; }
     const size_t n_in = static_cast<size_t>(in_w) * in_h;
     const bool rectify = (flags & MDC_RECTIFY) != 0;
     std::vector<size_t> level_px(static_cast<size_t>(levels));
-    for (int l = 0; l < levels; ++l)      // level l of getImage's result: (w >> l) x (h >> l), mdc_prepare_batch
+    for (int l = 0; l < levels; ++l) {      // level l of getImage's result: (w >> l) x (h >> l), mdc_prepare_batch
         level_px[static_cast<size_t>(l)] = static_cast<size_t>((rectify ? out_w : in_w) >> l) * static_cast<size_t>((rectify ? out_h : in_h) >> l);
+        if (!h_out_levels[l] && level_px[static_cast<size_t>(l)] > 0) {      // a level without pixels may be NULL, as for mdc_prepare_batch
+            mdc_set_error("mdc_seq_prepare: output level %d is NULL", l);
+            return MDC_ERR_INVALID_ARG;
+        }
+    }
+    if (count == 0) return MDC_OK;
     if (threads < 1) threads = default_decode_threads();
     // a chunk is what the GPU side takes at a time: two frames per decode thread (handed out dynamically, so a slow frame or a
     // descheduled thread does not hold the chunk up), small enough that the un-overlapped head (first decode) and tail (last
@@ -335,7 +349,9 @@ extern "C" int mdc_seq_prepare(mdc_ctx* c, const mdc_seq* s, int first, int coun
     for (auto& a : next_frame) a.store(0, std::memory_order_relaxed);
     int released = 1;                 // chunks whose buffer may be written: 0 .. released (stage[0] and stage[1] are free at the start)
     bool abort = false;
-    std::string first_error;
+    // first error met in chunk k.  Per chunk, because the workers run one chunk ahead: an error in chunk k+1 must not stop the call
+    // before chunk k, which decoded fine, has been prepared (the reference prepares every frame before the bad one).
+    std::vector<std::string> chunk_error(static_cast<size_t>(n_chunks));
     auto worker = [&](int) {
         std::vector<uint8_t> px;
         for (int k = 0; k < n_chunks; ++k) {
@@ -359,7 +375,7 @@ extern "C" int mdc_seq_prepare(mdc_ctx* c, const mdc_seq* s, int first, int coun
                 }
             }
             std::lock_guard<std::mutex> lk(mu);
-            if (!err.empty() && first_error.empty()) first_error = err;
+            if (!err.empty() && chunk_error[static_cast<size_t>(k)].empty()) chunk_error[static_cast<size_t>(k)] = err;
             ++decoded[static_cast<size_t>(k)];
             cv.notify_all();
         }
@@ -380,7 +396,7 @@ extern "C" int mdc_seq_prepare(mdc_ctx* c, const mdc_seq* s, int first, int coun
         {
             std::unique_lock<std::mutex> lk(mu);
             cv.wait(lk, [&] { return decoded[static_cast<size_t>(k)] == workers; });
-            err = first_error;
+            err = chunk_error[static_cast<size_t>(k)];
         }
         if (!err.empty()) {
             printf("ERROR: %s\n", err.c_str());

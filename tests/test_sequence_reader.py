@@ -150,7 +150,8 @@ def test_error_paths(tmp_path, capfd):
 @pytest.mark.gpu
 @pytest.mark.parametrize("zipped", [False, True], ids=["folder", "zip"])
 def test_decode_ahead_feed_matches_the_oracle(tmp_path, zipped):
-    """mdc_seq_prepare = decode (host threads) -> pinned staging -> H2D -> fused kernel -> D2H, 70 frames in chunks of 32."""
+    """mdc_seq_prepare = decode (host threads) -> pinned staging -> H2D -> fused kernel -> D2H, 65 frames in chunks of 16 (two per
+    decode thread, at least 16).  tests/test_sequence_feed.py pins the feed frame for frame on JPEG sequences."""
     from conftest import assert_bits_equal
     from oracle.loader import PortOracle
     port = PortOracle()
