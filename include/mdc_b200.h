@@ -231,8 +231,8 @@ int mdc_seq_prepare(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned
  * vignetteCalib optimiser, main_vignetteCalib.cpp:395-585 (SURVEY.md §8f N4).  Everything is device-resident, contiguous:
  *   d_images [n][wI*hI] float (NaN = invalidated pixel, :300-310), d_p2x / d_p2y [n][gw*gh] float plane-to-image maps
  *   (NaN = plane point not visible; finite entries keep the four bilinear taps inside the image, :352-356),
- *   d_plane_color [gw*gh], d_vignette [wI*hI].  The marker detection and cv::findHomography stay with the caller; the maps and
- *   images come from mdc_vc_plane_maps and mdc_vc_prepare_images below.
+ *   d_plane_color [gw*gh], d_vignette [wI*hI].  The homographies come from mdc_marker_detect and mdc_marker_homography below,
+ *   the maps and images from mdc_vc_plane_maps and mdc_vc_prepare_images.
  * Unlike the reference, which reads planeColor uninitialised in its first pass (:381, :425), the caller provides it.
  * With n = 0, d_images, d_p2x and d_p2y may be null; the plane colour and the vignette then become NaN, as in the reference.
  * integer_abs: the reference's outlier test is `abs(residual) > oth2` on a double (:423, :481).  1 = the residual is truncated to
@@ -285,6 +285,50 @@ int mdc_vc_plane_maps(const mdc_fov* fov, const double* homographies, int n, int
  * `stream` NULL = the context's stream, synchronised before returning. */
 int mdc_vc_prepare_images(mdc_ctx* c, const float* d_raw, int n, int wI, int hI, const float* exposures_host, float mean_exposure,
                           int max_abs_grad, float* d_images, mdc_stream stream);
+
+/* =====================================================================================
+ * vignetteCalib's marker detection and homography, main_vignetteCalib.cpp:231-253: aruco 1.3.0's MarkerDetector::detect with
+ * its default settings (aruco-1.3.0/src/markerdetector.cpp:50-64: ADPT_THRES 7/7, LINES corners, 56-pixel warp,
+ * FiducidalMarkers::detect) on the rectified frame rounded to 8 bits, then cv::findHomography from the unit square.  Paths
+ * below are inside aruco-1.3.0/src/.  The per-pixel passes run on the GPU (mdc_marker_threshold); the contour logic runs on the
+ * host, one frame per call, re-entrant (no shared state), so frames can go to as many host threads as there are.
+ * ===================================================================================== */
+typedef struct mdc_marker {
+    int id;             /* FiducidalMarkers id, 0..1023 */
+    float corners[8];   /* x0 y0 .. x3 y3 in rectified pixels, in the order aruco returns them (rotation applied) */
+} mdc_marker;
+/* main_vignetteCalib.cpp:235-236 (convertTo(CV_8U, 1, 0): round half to even, saturate; NaN -> 0) and markerdetector.cpp:437-458
+ * (adaptiveThreshold(grey, 255, ADAPTIVE_THRESH_MEAN_C, THRESH_BINARY_INV, 7, 7): the 7x7 mean with replicated image borders,
+ * rounded to 8 bits; mask = grey - mean <= -7 ? 255 : 0), batched and bit-identical to OpenCV for finite inputs below 2^31:
+ *   d_rect [n][h][w] f32 (mdc_prepare_batch level 0 with MDC_RECTIFY only), d_grey, d_mask [n][h][w] u8 (DEVICE pointers).
+ * Any 1 <= w, h with w*h <= 2^28; `stream` as for mdc_prepare_batch. */
+int mdc_marker_threshold(mdc_ctx* c, const float* d_rect, int n, int w, int h, uint8_t* d_grey, uint8_t* d_mask, mdc_stream stream);
+/* MarkerDetector::detect from there on (HOST pointers, w*h bytes each): detectRectangles (:287-430: findContours(CV_RETR_LIST,
+ * CV_CHAIN_APPROX_NONE) with the outer rows and columns as background, contour length filter, approxPolyDP to convex quads with
+ * sides > 10 px, anti-clockwise corners, too-near candidates), the id reader per candidate (:166-191, arucofidmarkers.cpp:290-465:
+ * perspective warp to 56 x 56, Otsu, 7 x 7 cells, Hamming code in four rotations), LINES corner refinement (:779-928) and the
+ * final filters (:218-253: one marker per id, the larger perimeter; none within 2.5 % of the image border).  *count = markers
+ * found; at most `capacity` are written, sorted by id; more than `capacity` returns MDC_ERR_INVALID_ARG.  Ids, candidates and
+ * warped patches are exact; the corners come from two least-squares solves done in double where aruco solves in fp32 by SVD,
+ * so they agree to about 1e-3 px.  Masks with more than 2^22 contours or 2^14 candidates return MDC_ERR_UNSUPPORTED. */
+int mdc_marker_detect(const uint8_t* grey, const uint8_t* mask, int w, int h, mdc_marker* out, int capacity, int* count);
+/* main_vignetteCalib.cpp:242-253: the homography H (row-major, H[8] = 1) that maps the plane points (-0.5, 0.5), (0.5, 0.5),
+ * (0.5, -0.5), (-0.5, -0.5) to corners 0..3, from the exact 8 x 8 system solved in double with partial pivoting (cv::findHomography
+ * gives the same to ~1e-13 relative for four points).  A quad with three corners on a line, or with a non-finite corner,
+ * returns MDC_ERR_INVALID_ARG. */
+int mdc_marker_homography(const float corners[8], double H[9]);
+/* The stages of mdc_marker_detect one by one, so that each can be checked against the OpenCV call it restates:
+ *   mdc_marker_contours     findContours's output: *n_contours contours of lengths[i] points each, xy = x, y pairs of all of
+ *                           them in findContours's order (last found first); capacities too small -> MDC_ERR_INVALID_ARG
+ *   mdc_marker_approx_poly  approxPolyDP(xy[0..n), eps, closed = true) into out_xy (room for n points)
+ *   mdc_marker_candidates   the candidates that detectRectangles returns (quads [count][8])
+ *   mdc_marker_read_patch   the 56 x 56 warped patch of a quad (before Otsu), the Otsu threshold, id (-1 = none) and rotations */
+int mdc_marker_contours(const uint8_t* mask, int w, int h, int* xy, size_t point_capacity, int* lengths, int contour_capacity,
+                        int* n_contours, size_t* n_points);
+int mdc_marker_approx_poly(const int* xy, int n, double eps, int* out_xy, int* n_out);
+int mdc_marker_candidates(const uint8_t* mask, int w, int h, float* quads, int capacity, int* count);
+int mdc_marker_read_patch(const uint8_t* grey, int w, int h, const float quad[8], uint8_t* patch, int* otsu_threshold, int* id,
+                          int* rotations);
 
 /* responseCalib E-step, main_responseCalib.cpp:317-346 (kernel K3):
  *   d_data [n][npix] u8 image-major, d_t [n] f64 exposure times, d_G [256] f64 -> d_E [npix] f64.

@@ -51,6 +51,13 @@ SIGNATURES = {
     "mdc_vignette_calib": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp, C.POINTER(C.c_double)]),
     "mdc_vc_plane_maps": (C.c_int, [_vp, C.POINTER(C.c_double), C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, _vp, _vp, C.c_int, _vp]),
     "mdc_vc_prepare_images": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, _f32p, C.c_float, C.c_int, _vp, _vp]),
+    "mdc_marker_threshold": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp]),
+    "mdc_marker_detect": (C.c_int, [_vp, _vp, C.c_int, C.c_int, _vp, C.c_int, C.POINTER(C.c_int)]),
+    "mdc_marker_homography": (C.c_int, [_f32p, C.POINTER(C.c_double)]),
+    "mdc_marker_contours": (C.c_int, [_vp, C.c_int, C.c_int, _vp, C.c_size_t, _vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_size_t)]),
+    "mdc_marker_approx_poly": (C.c_int, [_vp, C.c_int, C.c_double, _vp, C.POINTER(C.c_int)]),
+    "mdc_marker_candidates": (C.c_int, [_vp, C.c_int, C.c_int, _f32p, C.c_int, C.POINTER(C.c_int)]),
+    "mdc_marker_read_patch": (C.c_int, [_vp, C.c_int, C.c_int, _f32p, _vp, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "mdc_atanf_device": (C.c_int, [_vp, _vp, C.c_size_t, C.c_int, _vp]),
     "mdc_fov_remap_x": (_f32p, [_vp]),
     "mdc_fov_remap_y": (_f32p, [_vp]),

@@ -461,6 +461,20 @@ class Context:
         return smoothed, log[:max_iterations]
 
     # ---- host-buffer operators (numpy)
+    def marker_threshold(self, rect, grey=None, mask=None):
+        """vignetteCalib's 8-bit conversion and aruco's adaptive threshold on the GPU (mdc_marker_threshold): rect float32 CUDA tensor
+        [n, h, w] of rectified frames; grey, mask uint8 [n, h, w] (new tensors when None).  Returns (grey, mask)."""
+        import torch
+        n, h, w = rect.shape
+        grey = torch.empty(rect.shape, dtype=torch.uint8, device=rect.device) if grey is None else grey
+        mask = torch.empty(rect.shape, dtype=torch.uint8, device=rect.device) if mask is None else mask
+        assert rect.is_cuda and rect.dtype == torch.float32 and rect.is_contiguous()
+        for t_ in (grey, mask):
+            assert t_.is_cuda and t_.dtype == torch.uint8 and t_.is_contiguous() and tuple(t_.shape) == (n, h, w)
+        check(lib.mdc_marker_threshold(self._h, C.c_void_p(rect.data_ptr()), n, w, h, C.c_void_p(grey.data_ptr()),
+                                       C.c_void_p(mask.data_ptr()), self._stream(rect)), "mdc_marker_threshold")
+        return grey, mask
+
     def unmap_host(self, image_in: np.ndarray, image_out: np.ndarray, n, flags):
         assert image_in.dtype == np.uint8 and image_out.dtype == np.float32
         check(lib.mdc_unmap_u8_host(self._h, image_in.ctypes.data_as(C.c_void_p), image_out.ctypes.data_as(C.c_void_p), n, flags),
@@ -611,3 +625,78 @@ def atanf_device(x):
     check(lib.mdc_atanf_device(C.c_void_p(x.data_ptr()), C.c_void_p(out.data_ptr()), x.numel(), x.device.index or 0,
                                C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)), "mdc_atanf_device")
     return out
+
+
+class _Marker(C.Structure):
+    _fields_ = [("id", C.c_int), ("corners", C.c_float * 8)]
+
+
+def _u8_image(a, name):
+    a = np.ascontiguousarray(a, dtype=np.uint8)
+    assert a.ndim == 2, f"{name} must be [h, w]"
+    return a
+
+
+def marker_detect(grey: np.ndarray, mask: np.ndarray, capacity: int = 64):
+    """aruco's MarkerDetector::detect from the 8-bit frame and its threshold mask (mdc_marker_detect), both uint8 [h, w]:
+    a list of (id, corners float32 [4, 2]) sorted by id."""
+    grey, mask = _u8_image(grey, "grey"), _u8_image(mask, "mask")
+    assert grey.shape == mask.shape
+    h, w = grey.shape
+    out = (_Marker * max(capacity, 1))()
+    count = C.c_int()
+    check(lib.mdc_marker_detect(grey.ctypes.data, mask.ctypes.data, w, h, out, capacity, C.byref(count)), "mdc_marker_detect")
+    return [(out[i].id, np.array(out[i].corners, np.float32).reshape(4, 2)) for i in range(count.value)]
+
+
+def marker_homography(corners) -> np.ndarray:
+    """vignetteCalib's homography from the unit square to the four marker corners (mdc_marker_homography): float64 [3, 3]."""
+    c = np.ascontiguousarray(np.asarray(corners, np.float32).reshape(8))
+    H = (C.c_double * 9)()
+    check(lib.mdc_marker_homography(c.ctypes.data_as(_f32p), H), "mdc_marker_homography")
+    return np.array(H[:], np.float64).reshape(3, 3)
+
+
+def marker_contours(mask: np.ndarray):
+    """The contours mdc_marker_detect traces (mdc_marker_contours), in findContours's order: a list of int32 [n, 2] arrays (x, y)."""
+    mask = _u8_image(mask, "mask")
+    h, w = mask.shape
+    nc, npt = C.c_int(), C.c_size_t()
+    lib.mdc_marker_contours(mask.ctypes.data, w, h, None, 0, None, 0, C.byref(nc), C.byref(npt))
+    xy = np.empty((max(npt.value, 1), 2), np.int32)
+    lengths = np.empty(max(nc.value, 1), np.int32)
+    check(lib.mdc_marker_contours(mask.ctypes.data, w, h, xy.ctypes.data, npt.value, lengths.ctypes.data, nc.value, C.byref(nc),
+                                  C.byref(npt)), "mdc_marker_contours")
+    ends = np.cumsum(lengths[:nc.value])
+    return [xy[e - n:e].copy() for e, n in zip(ends, lengths[:nc.value])]
+
+
+def marker_approx_poly(points, eps: float) -> np.ndarray:
+    """approxPolyDP(points, eps, closed=True) as mdc_marker_detect computes it: int32 [m, 2]."""
+    p = np.ascontiguousarray(np.asarray(points, np.int32).reshape(-1, 2))
+    out = np.empty((max(len(p), 1), 2), np.int32)
+    n = C.c_int()
+    check(lib.mdc_marker_approx_poly(p.ctypes.data, len(p), float(eps), out.ctypes.data, C.byref(n)), "mdc_marker_approx_poly")
+    return out[:n.value].copy()
+
+
+def marker_candidates(mask: np.ndarray, capacity: int = 4096) -> np.ndarray:
+    """The quads detectRectangles keeps (mdc_marker_candidates): float32 [count, 4, 2]."""
+    mask = _u8_image(mask, "mask")
+    h, w = mask.shape
+    out = np.empty((max(capacity, 1), 4, 2), np.float32)
+    n = C.c_int()
+    check(lib.mdc_marker_candidates(mask.ctypes.data, w, h, out.ctypes.data_as(_f32p), capacity, C.byref(n)), "mdc_marker_candidates")
+    return out[:n.value].copy()
+
+
+def marker_read_patch(grey: np.ndarray, quad):
+    """The id reader on one quad (mdc_marker_read_patch): (warped 56x56 uint8 patch before Otsu, Otsu threshold, id or -1, rotations)."""
+    grey = _u8_image(grey, "grey")
+    h, w = grey.shape
+    q = np.ascontiguousarray(np.asarray(quad, np.float32).reshape(8))
+    patch = np.empty((56, 56), np.uint8)
+    t, i, r = C.c_int(), C.c_int(), C.c_int()
+    check(lib.mdc_marker_read_patch(grey.ctypes.data, w, h, q.ctypes.data_as(_f32p), patch.ctypes.data, C.byref(t), C.byref(i), C.byref(r)),
+          "mdc_marker_read_patch")
+    return patch, t.value, i.value, r.value

@@ -46,14 +46,14 @@ def build(force: bool = False, verbose: bool = False) -> str:
     os.makedirs(obj_dir, exist_ok=True)
     os.makedirs(LIB_DIR, exist_ok=True)
     objs, log, rebuilt = [], [], False
-    for src in ("mdc_host_models.cpp", "mdc_gray_image.cpp", "mdc_jpeg.cpp", "mdc_sequence.cpp"):
+    for src in ("mdc_host_models.cpp", "mdc_gray_image.cpp", "mdc_jpeg.cpp", "mdc_sequence.cpp", "mdc_marker.cpp"):
         o = os.path.join(obj_dir, src + ".o")
         s = os.path.join(CSRC, src)
         if force or _newer(o, [s] + headers):
             _run([gxx, "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-Wall", *inc, "-c", s, "-o", o], log)
             rebuilt = True
         objs.append(o)
-    for src in ("mdc_kernels.cu", "mdc_capi.cu", "mdc_vignette_calib.cu"):
+    for src in ("mdc_kernels.cu", "mdc_capi.cu", "mdc_vignette_calib.cu", "mdc_marker.cu"):
         o = os.path.join(obj_dir, src + ".o")
         s = os.path.join(CSRC, src)
         if force or _newer(o, [s] + headers):

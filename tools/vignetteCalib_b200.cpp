@@ -6,20 +6,25 @@
 // libmdc_b200.so: gamma removal (mdc_unmap_u8), exposure normalisation and gradient invalidation (mdc_vc_prepare_images),
 // projection + distortion + visibility mask of the plane grid (mdc_vc_plane_maps), and the loop (mdc_vignette_calib).
 //
-// The marker detection (aruco) and cv::findHomography are not part of the library.  Their result comes from a file instead:
-// nine whitespace-separated numbers (the row-major 3x3 homography from marker corners to rectified pixels) per considered frame
-// i = 0, skip, 2*skip, ...  A row containing NaN means that no marker was found in that frame: the frame is left out (:240),
-// but its exposure still counts in the mean exposure, as in the reference.  The debug overlays and imshow windows (:306-368) are
-// not produced.
+// The homographies from the unit square to the marker (:231-262) come from one of two places:
+//   homographies=detect  the tool detects the marker itself: raw frame -> rectification (mdc_prepare_batch, MDC_RECTIFY) -> 8-bit
+//                        frame and adaptive threshold (mdc_marker_threshold) on the GPU, in chunks of frames; then aruco's
+//                        detector (mdc_marker_detect) on host threads, one frame per thread, and mdc_marker_homography.  The rows
+//                        it used are written to vignetteCalibResult/homographies.txt, in the format homographies=FILE reads.
+//   homographies=FILE    nine whitespace-separated numbers (the row-major 3x3 homography from marker corners to rectified pixels)
+//                        per considered frame i = 0, skip, 2*skip, ...
+// A row containing NaN means that the frame does not show exactly one marker: the frame is left out (:240), but its exposure
+// still counts in the mean exposure, as in the reference.  The debug overlays and imshow windows (:306-368) are not produced.
 //
-//   vignetteCalib_b200 <dataset dir/> homographies=FILE [iterations=20] [skip=1] [patternX=1000] [patternY=1000] [facW=5] [facH=5]
-//                      [device=0]
+//   vignetteCalib_b200 <dataset dir/> homographies=FILE|detect [iterations=20] [skip=1] [patternX=1000] [patternY=1000] [facW=5]
+//                      [facH=5] [device=0]
 //
 // Build (see tests/test_vignette_calib_tool.py):  g++ -std=c++11 -O2 -Iinclude tools/vignetteCalib_b200.cpp
 //                                                 -Lmono_dataset_code_b200/lib -lmdc_b200 -L/usr/local/cuda/lib64 -lcudart -lz
 #include <cuda_runtime.h>
 #include <zlib.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstdint>
 #include <cstdio>
@@ -27,6 +32,7 @@
 #include <cstring>
 #include <fstream>
 #include <string>
+#include <thread>
 #include <vector>
 
 #include "mdc_b200.h"
@@ -129,18 +135,79 @@ bool write_plane_png(const std::string& path, const std::vector<float>& I, int w
     return write_png(path, px, w, h, 8, 2);
 }
 
+// Homographies of frames i = 0, skip, ... by marker detection; writes them (NaN rows for frames without exactly one marker) to `out`.
+void detect_homographies(mdc_ctx* ctx, mdc_seq* seq, int skip, int wI, int hI, int w_out, int h_out, const char* out) {
+    const int num_images = mdc_seq_num_images(seq);
+    std::vector<int> ids;
+    for (int i = 0; i < num_images; i += skip) ids.push_back(i);
+    const size_t npx_in = static_cast<size_t>(wI) * hI, npx = static_cast<size_t>(w_out) * h_out;
+    const int chunk = static_cast<int>(std::max<size_t>(1, std::min<size_t>(32, (size_t(1) << 30) / (npx * 4 + npx_in))));
+    std::vector<uint8_t> raw(chunk * npx_in), grey(chunk * npx), mask(chunk * npx);
+    uint8_t *d_raw = nullptr, *d_grey = nullptr, *d_mask = nullptr;
+    float* d_rect = nullptr;
+    CUDA_OR_DIE(cudaMalloc(&d_raw, raw.size()));
+    CUDA_OR_DIE(cudaMalloc(&d_rect, chunk * npx * sizeof(float)));
+    CUDA_OR_DIE(cudaMalloc(&d_grey, grey.size()));
+    CUDA_OR_DIE(cudaMalloc(&d_mask, mask.size()));
+    std::vector<double> Hs(ids.size() * 9, NAN);
+    const int threads = std::max(1u, std::thread::hardware_concurrency());
+    int found = 0;
+    for (size_t first = 0; first < ids.size(); first += chunk) {
+        const int m = static_cast<int>(std::min<size_t>(chunk, ids.size() - first));
+        for (int k = 0; k < m; ++k) {
+            int fw = 0, fh = 0;
+            if (mdc_seq_read_gray8(seq, ids[first + k], raw.data() + k * npx_in, npx_in, &fw, &fh) != MDC_OK || fw != wI || fh != hI) {
+                printf("frame %d: cannot read a %dx%d image: %s\n", ids[first + k], wI, hI, mdc_last_error());
+                exit(1);
+            }
+        }
+        CUDA_OR_DIE(cudaMemcpy(d_raw, raw.data(), m * npx_in, cudaMemcpyHostToDevice));
+        MDC_OR_DIE(mdc_prepare_batch(ctx, d_raw, m, MDC_RECTIFY, &d_rect, 1, nullptr));           // getImage(i, true, false, false, false)
+        MDC_OR_DIE(mdc_marker_threshold(ctx, d_rect, m, w_out, h_out, d_grey, d_mask, nullptr));
+        CUDA_OR_DIE(cudaMemcpy(grey.data(), d_grey, m * npx, cudaMemcpyDeviceToHost));
+        CUDA_OR_DIE(cudaMemcpy(mask.data(), d_mask, m * npx, cudaMemcpyDeviceToHost));
+        std::vector<int> status(m, MDC_OK);
+        std::vector<std::string> errors(m);
+        std::vector<std::thread> pool;
+        for (int t = 0; t < std::min(threads, m); ++t)
+            pool.emplace_back([&, t]() {
+                for (int k = t; k < m; k += threads) {
+                    mdc_marker markers[2];
+                    int count = 0;
+                    status[k] = mdc_marker_detect(grey.data() + k * npx, mask.data() + k * npx, w_out, h_out, markers, 2, &count);
+                    if (status[k] == MDC_ERR_INVALID_ARG && count > 2) status[k] = MDC_OK;    // more than one marker: skipped (:240)
+                    if (status[k] != MDC_OK) { errors[k] = mdc_last_error(); continue; }
+                    if (count == 1 && mdc_marker_homography(markers[0].corners, &Hs[(first + k) * 9]) != MDC_OK)
+                        for (int q = 0; q < 9; ++q) Hs[(first + k) * 9 + q] = NAN;
+                }
+            });
+        for (std::thread& t : pool) t.join();
+        for (int k = 0; k < m; ++k) {
+            if (status[k] != MDC_OK) { printf("frame %d: marker detection failed: %s\n", ids[first + k], errors[k].c_str()); exit(2); }
+            found += !std::isnan(Hs[(first + k) * 9]);
+        }
+    }
+    cudaFree(d_raw); cudaFree(d_rect); cudaFree(d_grey); cudaFree(d_mask);
+    printf("found exactly one marker in %d of %zu frames\n", found, ids.size());
+    FILE* f = fopen(out, "w");
+    if (!f) { printf("cannot write %s\n", out); exit(1); }
+    for (size_t r = 0; r < ids.size(); ++r)
+        for (int q = 0; q < 9; ++q) fprintf(f, "%.17g%c", Hs[r * 9 + q], q == 8 ? '\n' : ' ');
+    if (fclose(f) != 0) { printf("cannot write %s\n", out); exit(1); }
+}
+
 }  // namespace
 
 int main(int argc, char** argv) {
     if (argc < 2) {
-        printf("usage: vignetteCalib_b200 <dataset dir/> homographies=FILE [iterations=N] [skip=N] [patternX=N] [patternY=N] [facW=F] [facH=F] "
+        printf("usage: vignetteCalib_b200 <dataset dir/> homographies=FILE|detect [iterations=N] [skip=N] [patternX=N] [patternY=N] [facW=F] [facH=F] "
                "[device=N]\n");
         return 1;
     }
     Options opt;
     for (int i = 2; i < argc; ++i) parse_option(argv[i], &opt);
     if (opt.skip < 1) opt.skip = 1;
-    if (opt.homographies.empty()) { printf("homographies=FILE is required\n"); return 1; }
+    if (opt.homographies.empty()) { printf("homographies=FILE is required (or homographies=detect)\n"); return 1; }
     if (opt.gw < 1 || opt.gh < 1) { printf("patternX / patternY must be positive\n"); return 1; }
 
     if (system("rm -rf vignetteCalibResult") == -1) printf("could not delete old vignetteCalibResult folder!\n");
@@ -164,6 +231,14 @@ int main(int argc, char** argv) {
     for (int i = 0; i < num_images; i += opt.skip) mean_exposure += mdc_seq_exposure(seq, i);
     mean_exposure = mean_exposure / num_images;
     if (mean_exposure == 0) mean_exposure = 1;
+
+    CUDA_OR_DIE(cudaSetDevice(opt.device));
+    mdc_ctx* ctx = nullptr;
+    MDC_OR_DIE(mdc_ctx_create(opt.device, fov, photo, &ctx));
+    if (opt.homographies == "detect") {
+        opt.homographies = "vignetteCalibResult/homographies.txt";
+        detect_homographies(ctx, seq, opt.skip, wI, hI, w_out, h_out, opt.homographies.c_str());
+    }
 
     // ---- frames that have a homography
     FILE* hf = fopen(opt.homographies.c_str(), "r");
@@ -194,9 +269,6 @@ int main(int argc, char** argv) {
     const size_t gwgh = static_cast<size_t>(opt.gw) * opt.gh;
 
     // ---- front end on the device: gamma removal, normalisation + gradient invalidation, plane-to-image maps
-    CUDA_OR_DIE(cudaSetDevice(opt.device));
-    mdc_ctx* ctx = nullptr;
-    MDC_OR_DIE(mdc_ctx_create(opt.device, fov, photo, &ctx));
     uint8_t* d_frames = nullptr;
     float *d_images = nullptr, *d_p2x = nullptr, *d_p2y = nullptr, *d_plane = nullptr, *d_vig = nullptr, *d_smoothed = nullptr;
     CUDA_OR_DIE(cudaMalloc(&d_images, npx * n * sizeof(float) + 4));
