@@ -346,7 +346,9 @@ int mdc_estep(mdc_ctx* c, const uint8_t* d_data, int n, int npix, const double* 
  *                        below the largest one (and below 2^1024 when max|E| * max|t| overflows).  Non-finite products (an
  *                        overflowing E*t, a NaN or infinite E or t) are summed in fp64 on the side and poison their bins as in
  *                        the reference; a non-finite exposure time of a fully saturated frame changes nothing, as in the reference.
- *                        With n = 0, d_data and d_t may be null (also for mdc_estep, mdc_rc_einit and mdc_rc_rmse).
+ *                        With n = 0, d_data and d_t may be null (also for mdc_estep, mdc_rc_einit and mdc_rc_rmse).  With npix = 0
+ *                        (the empty slice of a pixel-sharded rank), mdc_estep, mdc_rc_einit and mdc_rc_rescale accept null d_data
+ *                        and d_E and touch neither.
  *   mdc_rc_rescale       factor = 255/G[255]; E *= factor; G *= factor; *factor_host = factor           :350-355                       bit-exact
  *   mdc_rc_rmse          out_host = {1e5*sqrt(mean((G[b]-t*E)^2 * 1e-10)), count}                       :50-69                         rounding-level
  *                        (the reference sums in long double); residuals, finite test and count exact; same bits on every run.

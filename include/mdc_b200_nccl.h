@@ -33,7 +33,11 @@ int mdc_nccl_version(void);
  * _accumulate_exact / _finish_exact, include/mdc_b200.h): per iteration ncclAllReduce MAX of 4 u64, SUM of 768 int64 and of 256 fp64
  * (+ 256 u64 counts in the first iteration), so d_G and d_E_local hold the same bits for ANY number of ranks, mdc_response_calib's
  * included; the three rmse evaluations all-reduce 2 doubles each; E-step, E-init and rescale are collective-free.  log_host as in
- * mdc_response_calib (global rmse / count).  Same call on every rank. */
+ * mdc_response_calib (global rmse / count).  Same call on every rank.  A rank may hold no pixels (npix_local = 0; d_data_local and
+ * d_E_local may then be null): it still takes part in every collective.
+ * A rank that fails mid-loop (a CUDA error, a bad argument on that rank only) returns without reaching the remaining collectives, and
+ * its peers then wait in an all-reduce that never completes: NCCL has no timeout here, so the host must abort the communicator
+ * (ncclCommAbort) or end the processes.  The call does not recover from that. */
 int mdc_response_calib_sharded(mdc_ctx* c, void* nccl_comm, int device, const uint8_t* d_data_local, int n, int npix_local,
                                const double* d_t, int nits, double* d_E_local, double* d_G, double* log_host);
 

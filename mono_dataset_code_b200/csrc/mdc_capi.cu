@@ -990,7 +990,11 @@ void mdc_ctx_add_launches(mdc_ctx* c, int n) { c->launches += n; }
 void mdc_ctx_geometry(const mdc_ctx* c, int* in_w, int* in_h, int* out_w, int* out_h) { *in_w = c->in_w; *in_h = c->in_h; *out_w = c->out_w; *out_h = c->out_h; }
 
 extern "C" int mdc_estep(mdc_ctx* c, const uint8_t* d_data, int n, int npix, const double* d_t, const double* d_G, double* d_E, mdc_stream stream) {
-    if (!c || (n > 0 && (!d_data || !d_t)) || !d_G || !d_E || n < 0 || npix < 0) { mdc_set_error("mdc_estep: bad argument"); return MDC_ERR_INVALID_ARG; }
+    // an empty pixel slice (npix = 0, e.g. a rank of a pixel-sharded run) reads no data and writes no E: both may be null
+    if (!c || (n > 0 && ((npix > 0 && !d_data) || !d_t)) || !d_G || (npix > 0 && !d_E) || n < 0 || npix < 0) {
+        mdc_set_error("mdc_estep: bad argument");
+        return MDC_ERR_INVALID_ARG;
+    }
     CU_CHECK(cudaSetDevice(c->device));
     cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
     CU_CHECK(launch_estep(d_data, n, npix, d_t, d_G, d_E, s));
@@ -1019,7 +1023,7 @@ extern "C" int mdc_rc_leak_padding(mdc_ctx* c, uint8_t* d_data, int n, int w, in
 }
 
 extern "C" int mdc_rc_einit(mdc_ctx* c, const uint8_t* d_data, int n, int npix, double* d_E, mdc_stream stream) {
-    if (!c || (n > 0 && !d_data) || !d_E || n < 0 || npix < 0) { mdc_set_error("mdc_rc_einit: bad argument"); return MDC_ERR_INVALID_ARG; }
+    if (!c || (n > 0 && npix > 0 && !d_data) || (npix > 0 && !d_E) || n < 0 || npix < 0) { mdc_set_error("mdc_rc_einit: bad argument"); return MDC_ERR_INVALID_ARG; }
     CU_CHECK(cudaSetDevice(c->device));
     cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
     if (npix > 0) { CU_CHECK(launch_rc_einit(d_data, n, npix, d_E, s)); c->launches++; }
@@ -1117,9 +1121,9 @@ extern "C" int mdc_rc_rmse_accumulate(mdc_ctx* c, const uint8_t* d_data, int n, 
 }
 
 extern "C" int mdc_rc_rescale(mdc_ctx* c, int npix, double* d_E, double* d_G, double* factor_host) {
-    if (!c || !d_E || !d_G || npix < 0) { mdc_set_error("mdc_rc_rescale: bad argument"); return MDC_ERR_INVALID_ARG; }
+    if (!c || (npix > 0 && !d_E) || !d_G || npix < 0) { mdc_set_error("mdc_rc_rescale: bad argument"); return MDC_ERR_INVALID_ARG; }
     CU_CHECK(cudaSetDevice(c->device));
-    CU_CHECK(launch_rc_rescale(npix, d_E, d_G, c->d_rc + 512, c->stream));
+    CU_CHECK(launch_rc_rescale(npix, d_E, d_G, c->d_rc + 512, c->stream));      // with npix = 0 the E launch touches nothing
     c->launches += 3;
     if (factor_host) CU_CHECK(cudaMemcpyAsync(factor_host, c->d_rc + 512, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
     CU_CHECK(cudaStreamSynchronize(c->stream));

@@ -134,7 +134,8 @@ extern "C" int mdc_response_calib_sharded(mdc_ctx* c, void* nccl_comm, int devic
         }
         reusable = flag != 0;
     }
-    if (npix_local > 0) rc = mdc_rc_einit(c, d_data_local, n, npix_local, d_E_local, s);
+    // every per-rank call accepts an empty slice (npix_local = 0, null data and E), so every rank makes the same calls and collectives
+    rc = mdc_rc_einit(c, d_data_local, n, npix_local, d_E_local, s);
     if (rc == MDC_OK && cudaMemsetAsync(d_G, 0, 256 * sizeof(double), s) != cudaSuccess) rc = MDC_ERR_CUDA;
     for (int it = 0; it < nits && rc == MDC_OK; ++it) {
         double r[2], row[4] = {0, 0, 0, 0};
@@ -150,7 +151,7 @@ extern "C" int mdc_response_calib_sharded(mdc_ctx* c, void* nccl_comm, int devic
         if ((rc = mdc_rc_gstep_finish_exact(c, scale, limbs, special, gnum, d_G, s)) != MDC_OK) break;
         if ((rc = rmse(r)) != MDC_OK) break;
         row[0] = r[0];
-        if (npix_local > 0 && (rc = mdc_estep(c, d_data_local, n, npix_local, d_t, d_G, d_E_local, s)) != MDC_OK) break;
+        if ((rc = mdc_estep(c, d_data_local, n, npix_local, d_t, d_G, d_E_local, s)) != MDC_OK) break;
         if ((rc = rmse(r)) != MDC_OK) break;
         row[1] = r[0];
         // rescale (:350-355): the factor comes from the replicated G, so every rank applies the same one to its slice and to its G
