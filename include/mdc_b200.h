@@ -226,6 +226,24 @@ int mdc_seq_read_gray8(const mdc_seq* s, int id, uint8_t* out, size_t capacity, 
  * rows from that chunk on are not written.  first / count outside the sequence, levels outside 1..MDC_MAX_PYR_LEVELS or a NULL
  * level that has pixels (a level without pixels may be NULL) return MDC_ERR_INVALID_ARG before anything is decoded. */
 int mdc_seq_prepare(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned flags, float* const* h_out_levels, int levels, int threads);
+/* The same getImage for [first, first+count) into DEVICE level buffers (level l: [count][(w>>l)*(h>>l)] floats), with the JPEG frames
+ * decoded on the GPU: `threads` host threads (0 = all) read the files, parse the JPEG headers and split the scans into restart intervals,
+ * and the main thread packs the entropy-coded bytes of a chunk into pinned staging; each chunk then goes H2D -> entropy decode (J1) ->
+ * inverse DCT (J2) -> fused kernel (K1) on `stream` (NULL = the context's stream).  A chunk holds min(512, max(16, 32 * threads))
+ * frames; the host side of chunk k+1 overlaps the GPU side of chunk k.  PNG and PGM frames are decoded on the host and copied as
+ * 8-bit pixels.  The result equals mdc_seq_prepare's bit for bit, and so do the argument checks, the wrong-size rule and the error
+ * rule: a frame that cannot be decoded (on the host or on the GPU) stops the call with MDC_ERR_FORMAT, the chunks before its chunk
+ * are complete, and nothing from its chunk on is written.  Returns when the work is done on the device. */
+int mdc_seq_prepare_device(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned flags, float* const* d_out_levels, int levels,
+                           int threads, mdc_stream stream);
+/* Baseline JPEGs in HOST memory (files[i], sizes[i] bytes) -> 8-bit grey planes on the device, the same bytes as mdc_seq_read_gray8
+ * (the host decoder): d_out is [n][h][row_pitch] (row_pitch >= w; a multiple of 16 keeps mdc_prepare_batch_pitched on its TMA
+ * loader).  Headers are parsed on the host; a frame the parser rejects, or one that is not w x h, is never uploaded, and the frames
+ * around it still decode.  status_host (n ints, may be NULL) gets MDC_OK or MDC_ERR_FORMAT per frame; the call returns
+ * MDC_ERR_FORMAT if any frame failed, with the host decoder's message for the first one ("frame <i>: ..."), and leaves the rows of
+ * failed frames untouched.  Uses the context's device; `stream` as for mdc_prepare_batch; returns when the frames are decoded. */
+int mdc_jpeg_decode_device(mdc_ctx* c, const uint8_t* const* files, const size_t* sizes, int n, int w, int h, uint8_t* d_out,
+                           size_t row_pitch, int* status_host, mdc_stream stream);
 
 /* =====================================================================================
  * vignetteCalib optimiser, main_vignetteCalib.cpp:395-585 (SURVEY.md §8f N4).  Everything is device-resident, contiguous:

@@ -45,6 +45,9 @@ SIGNATURES = {
     "mdc_seq_exposure": (C.c_float, [_vp, C.c_int]),
     "mdc_seq_read_gray8": (C.c_int, [_vp, C.c_int, _vp, C.c_size_t, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "mdc_seq_prepare": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint, C.POINTER(_vp), C.c_int, C.c_int]),
+    "mdc_seq_prepare_device": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint, C.POINTER(_vp), C.c_int, C.c_int, _vp]),
+    "mdc_jpeg_decode_device": (C.c_int, [_vp, C.POINTER(_vp), C.POINTER(C.c_size_t), C.c_int, C.c_int, C.c_int, _vp, C.c_size_t,
+                                         C.POINTER(C.c_int), _vp]),
     "mdc_vc_plane_step": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _vp, _vp, C.c_double, C.c_int, C.POINTER(C.c_double)]),
     "mdc_vc_vignette_step": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _vp, _vp, C.c_double, C.c_int, C.POINTER(C.c_double)]),
     "mdc_vc_smooth": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, _vp]),

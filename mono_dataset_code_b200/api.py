@@ -240,6 +240,12 @@ class Context:
         self._h = h
         self.device = device
         self.fov, self.photo = fov, photo
+        if _adopt is not None:
+            self.in_dims = tuple(_adopt[0][:2])
+        elif fov is not None:
+            self.in_dims = tuple(fov.getInputDims())
+        else:
+            self.in_dims = (photo.w, photo.h) if photo is not None else (0, 0)
 
     @classmethod
     def from_device_tables(cls, device, in_w, in_h, out_w, out_h, rx, ry, ginv, vinv):
@@ -561,6 +567,20 @@ class Sequence:
               "mdc_seq_prepare")
         return outs
 
+    def prepare_device(self, ctx: "Context", first: int, count: int, rectify, removeGamma, removeVignette, nanOverexposed, levels: int = 1,
+                       threads: int = 0, out=None):
+        """getImage for frames [first, first+count) with the JPEG frames decoded on the GPU (mdc_seq_prepare_device) -> list of float32
+        CUDA tensors [count, w_l*h_l] on the context's device, one per pyramid level.  Runs on torch's current stream."""
+        import torch
+        if out is None:
+            w, h = ctx.level_dims(0) if rectify else ctx.in_dims
+            out = [torch.empty((count, (w >> l) * (h >> l)), dtype=torch.float32, device=f"cuda:{ctx.device}") for l in range(levels)]
+        ptrs = (C.c_void_p * len(out))(*[t.data_ptr() for t in out])
+        stream = Context._stream(out[0]) if out else None
+        check(lib.mdc_seq_prepare_device(ctx._h, self._h, first, count, _flags(rectify, removeGamma, removeVignette, nanOverexposed), ptrs,
+                                         len(out), threads, stream), "mdc_seq_prepare_device")
+        return out
+
 
 class FramePreparer:
     """The getImage composition of DatasetReader (BenchmarkDatasetReader.h:188-243) over frames that are already decoded
@@ -607,6 +627,27 @@ class FramePreparer:
             out = [torch.empty((n, w * h), dtype=torch.float32, device=frames.device) for (w, h) in self.level_shapes(rectify, levels)]
         self.ctx.prepare_batch(frames, _flags(rectify, removeGamma, removeVignette, nanOverexposed), out)
         return out
+
+
+def jpeg_decode_device(blobs, w: int, h: int, ctx: "Context | None" = None, device: int = 0, row_pitch: int | None = None, out=None):
+    """Baseline JPEG files (bytes) -> uint8 CUDA tensor [n, h, row_pitch] of grey planes decoded on the GPU (mdc_jpeg_decode_device), the
+    same bytes as the host decoder, and the per-frame status (0 = decoded, 3 = MDC_ERR_FORMAT: that frame's rows are left as they were).
+    row_pitch defaults to w rounded up to 16 bytes.  Errors other than undecodable frames raise MdcError."""
+    import torch
+    if ctx is None:
+        ctx = Context(None, None, device)
+    n = len(blobs)
+    pitch = row_pitch if row_pitch is not None else (w + 15) // 16 * 16
+    if out is None:
+        out = torch.zeros((n, h, pitch), dtype=torch.uint8, device=f"cuda:{ctx.device}")
+    keep = [bytes(b) for b in blobs]
+    files = (C.c_void_p * max(n, 1))(*[C.cast(C.c_char_p(b), C.c_void_p).value for b in keep])
+    sizes = (C.c_size_t * max(n, 1))(*[len(b) for b in keep])
+    status = (C.c_int * max(n, 1))()
+    rc = lib.mdc_jpeg_decode_device(ctx._h, files, sizes, n, w, h, C.c_void_p(out.data_ptr()), pitch, status, Context._stream(out))
+    if rc not in (0, 3):
+        check(rc, "mdc_jpeg_decode_device")
+    return out, np.array(status[:n], dtype=np.int32)
 
 
 def atanf_host(x: np.ndarray) -> np.ndarray:

@@ -150,17 +150,21 @@ bool mdc_decode_gray_image(const std::vector<uint8_t>& file, const std::string& 
     }
 }
 
+bool mdc_read_file(const std::string& path, std::vector<uint8_t>* file) {
+    std::ifstream f(path.c_str(), std::ios::binary | std::ios::ate);
+    if (!f.good()) { mdc_set_error("cannot open image %s", path.c_str()); return false; }
+    const std::streamoff size = f.tellg();
+    if (size < 0) { mdc_set_error("cannot read image %s", path.c_str()); return false; }
+    file->resize(static_cast<size_t>(size));
+    f.seekg(0);
+    if (size > 0 && !f.read(reinterpret_cast<char*>(file->data()), size)) { mdc_set_error("cannot read image %s", path.c_str()); return false; }
+    return true;
+}
+
 bool mdc_read_gray_image(const std::string& path, mdc_gray_image* out) {
     try {
-        std::ifstream f(path.c_str(), std::ios::binary | std::ios::ate);
-        if (!f.good()) { mdc_set_error("cannot open image %s", path.c_str()); return false; }
         static thread_local std::vector<uint8_t> file;      // per-thread scratch, read in one go (see mdc_jpeg.cpp on why not per frame)
-        const std::streamoff size = f.tellg();
-        if (size < 0) { mdc_set_error("cannot read image %s", path.c_str()); return false; }
-        file.resize(static_cast<size_t>(size));
-        f.seekg(0);
-        if (size > 0 && !f.read(reinterpret_cast<char*>(file.data()), size)) { mdc_set_error("cannot read image %s", path.c_str()); return false; }
-        return mdc_decode_gray_image(file, path, out);
+        return mdc_read_file(path, &file) && mdc_decode_gray_image(file, path, out);
     } catch (const std::exception& e) {
         mdc_set_error("%s: cannot read (%s)", path.c_str(), e.what());
         return false;

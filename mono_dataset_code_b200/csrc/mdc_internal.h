@@ -1,6 +1,7 @@
 // Internal declarations shared by the host-model, C-ABI and kernel translation units.
 #pragma once
 #include <stdint.h>
+#include <mutex>
 #include <string>
 #include <vector>
 
@@ -38,6 +39,7 @@ struct mdc_gray_image {
     std::vector<uint8_t> px;
 };
 bool mdc_read_gray_image(const std::string& path, mdc_gray_image* out);
+bool mdc_read_file(const std::string& path, std::vector<uint8_t>* file);                                        // whole file, undecoded
 bool mdc_decode_gray_image(const std::vector<uint8_t>& file, const std::string& name, mdc_gray_image* out);      // same, from memory
 bool mdc_decode_jpeg_gray(const std::vector<uint8_t>& file, const std::string& name, mdc_gray_image* out);       // baseline JPEG -> luminance (mdc_jpeg.cpp)
 
@@ -55,3 +57,10 @@ int mdc_ctx_device_ordinal(const mdc_ctx* c);
 void* mdc_ctx_stream_handle(mdc_ctx* c);          // the context's own cudaStream_t
 void mdc_ctx_add_launches(mdc_ctx* c, int n);
 void mdc_ctx_geometry(const mdc_ctx* c, int* in_w, int* in_h, int* out_w, int* out_h);
+
+// Sequence internals used by the GPU-decoding feed (mdc_jpeg_gpu.cu).
+struct mdc_seq_feed_stage { void* pinned[2] = {nullptr, nullptr}; size_t bytes[2] = {0, 0}; };      // pinned, kept between calls
+bool mdc_seq_read_file(const mdc_seq* s, int id, std::vector<uint8_t>* file);      // frame id's file bytes (folder file or zip entry)
+std::mutex& mdc_seq_feed_mutex(const mdc_seq* s);                                   // one feed at a time per sequence object
+mdc_seq_feed_stage* mdc_seq_device_stage(const mdc_seq* s);
+int mdc_seq_default_threads();                                                      // threads = 0 of the feeds

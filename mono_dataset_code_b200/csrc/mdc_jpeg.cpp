@@ -19,71 +19,16 @@
 #include <vector>
 
 #include "mdc_internal.h"
+#include "mdc_jpeg.h"
 #if defined(__x86_64__) && defined(__GNUC__)
 #include <immintrin.h>
 #endif
 
 namespace {
 
-constexpr int kLookBits = 9;      // Huffman codes up to this length are resolved by one table look-up
-constexpr int kFastBits = 10;     // window of the combined code + magnitude look-up of the AC tables
-
-struct HuffTable {
-    bool defined = false;
-    uint8_t bits[17] = {0};
-    uint8_t vals[256] = {0};
-    // canonical decoding tables (T.81 Annex F.2.2.3) + a prefix table for the short codes
-    int mincode[17], maxcode[18], valptr[17];
-    uint16_t look[1 << kLookBits];      // (code length << 8) | symbol, 0 = longer than kLookBits
-    // AC tables: a kFastBits-wide window resolves in one look-up every code that fits it TOGETHER with its magnitude bits, and the
-    // two symbols without magnitude bits: entry = (value << 16) | (kind << 9) | (run << 5) | total bits consumed;
-    // kind 0 = not covered (general path), 1 = coefficient, 2 = end of block, 3 = run of 16 zeros
-    int32_t fast[1 << kFastBits];
-    void build_fast() {
-        memset(fast, 0, sizeof fast);
-        int code = 0, k = 0;
-        for (int l = 1; l <= 16; ++l) {
-            for (int i = 0; i < bits[l]; ++i, ++code, ++k) {
-                if (l > kFastBits) continue;
-                const int run = vals[k] >> 4, mag = vals[k] & 15, spare = kFastBits - l;
-                for (int suffix = 0; suffix < (1 << spare); ++suffix) {
-                    int32_t e = 0;
-                    if (mag == 0) {
-                        e = ((run == 15 ? 3 : 2) << 9) | l;            // anything but ZRL ends the block, like the general path
-                    } else if (mag <= spare) {
-                        int v = suffix >> (spare - mag);                // the magnitude bits that follow the code
-                        if (v < (1 << (mag - 1))) v += 1 - (1 << mag);  // T.81 F.2.2.1 EXTEND
-                        e = (v * 65536) | (1 << 9) | (run << 5) | (l + mag);
-                    }
-                    fast[(code << spare) | suffix] = e;
-                }
-            }
-            code <<= 1;
-        }
-    }
-    // false = over-subscribed table (more codes of some length than the prefix code space has left; libjpeg's
-    // JERR_BAD_HUFF_TABLE).  Must be checked before look[] / fast[] are filled: such a table would index past their end.
-    bool build() {
-        int code = 0, k = 0;
-        memset(look, 0, sizeof look);
-        for (int l = 1; l <= 16; ++l) {
-            if (code + bits[l] > (1 << l)) return false;
-            valptr[l] = k;
-            mincode[l] = code;
-            for (int i = 0; i < bits[l]; ++i, ++code, ++k)
-                if (l <= kLookBits) {
-                    const int first = code << (kLookBits - l), span = 1 << (kLookBits - l);
-                    for (int j = 0; j < span; ++j) look[first + j] = static_cast<uint16_t>((l << 8) | vals[k]);
-                }
-            maxcode[l] = bits[l] ? code - 1 : -1;
-            code <<= 1;
-        }
-        maxcode[17] = 0x7fffffff;
-        return true;
-    }
-};
-
-struct Component { int id = 0, h = 1, v = 1, tq = 0, td = 0, ta = 0, pred = 0; };
+using mdcj::HuffTable;
+using mdcj::kLookBits;
+using mdcj::kFastBits;
 
 struct BitReader {
     const uint8_t* p;
@@ -149,8 +94,7 @@ inline int decode_symbol(BitReader& br, const HuffTable& t) {
 // T.81 F.2.2.1 EXTEND
 inline int extend(int v, int t) { return (t && v < (1 << (t - 1))) ? v - (1 << t) + 1 : v; }
 
-const uint8_t kZigZag[64] = {0, 1, 8, 16, 9, 2, 3, 10, 17, 24, 32, 25, 18, 11, 4, 5, 12, 19, 26, 33, 40, 48, 41, 34, 27, 20, 13, 6, 7, 14, 21, 28,
-                             35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51, 58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
+const uint8_t kZigZag[64] = MDC_JPEG_ZIGZAG;
 
 // One block: DC difference, then AC coefficients until end of block.  kStore = false for components that are only skipped (chroma of a
 // colour file): same bits consumed, nothing written.  The bit reader is copied into a local so that its state lives in registers (a
@@ -199,68 +143,12 @@ inline int decode_block(BitReader& reader, const HuffTable& dct, const HuffTable
     return any_ac;
 }
 
-// ---- inverse DCT, accurate integer method (13-bit constants, 2 guard bits between the passes)
-// Temporaries are 64-bit like libjpeg's (its JLONG is `long`), so no input — not even a corrupt one — can overflow.
-typedef int64_t wide;
-constexpr int kConstBits = 13, kPass1Bits = 2;
-constexpr wide F_0_298631336 = 2446, F_0_390180644 = 3196, F_0_541196100 = 4433, F_0_765366865 = 6270, F_0_899976223 = 7373,
-               F_1_175875602 = 9633, F_1_501321110 = 12299, F_1_847759065 = 15137, F_1_961570560 = 16069, F_2_053119869 = 16819,
-               F_2_562915447 = 20995, F_3_072711026 = 25172;
-inline wide descale(wide x, int n) { return (x + (wide(1) << (n - 1))) >> n; }      // arithmetic shift (floor), as in libjpeg
-inline uint8_t clamp_sample(wide v) { v += 128; return static_cast<uint8_t>(v < 0 ? 0 : (v > 255 ? 255 : v)); }
-
-struct Butterfly { wide e0, e1, e2, e3, o0, o1, o2, o3; };      // out[k] = e_k + o_(3-k), out[7-k] = e_k - o_(3-k)
-inline Butterfly idct_1d(wide c0, wide c1, wide c2, wide c3, wide c4, wide c5, wide c6, wide c7) {
-    Butterfly r;
-    // even part
-    wide z1 = (c2 + c6) * F_0_541196100;
-    const wide t2 = z1 + c6 * (-F_1_847759065), t3 = z1 + c2 * F_0_765366865;
-    const wide t0 = (c0 + c4) * (wide(1) << kConstBits), t1 = (c0 - c4) * (wide(1) << kConstBits);
-    r.e0 = t0 + t3; r.e3 = t0 - t3; r.e1 = t1 + t2; r.e2 = t1 - t2;
-    // odd part
-    wide a0 = c7, a1 = c5, a2 = c3, a3 = c1;
-    z1 = a0 + a3;
-    wide z2 = a1 + a2, z3 = a0 + a2, z4 = a1 + a3;
-    const wide z5 = (z3 + z4) * F_1_175875602;
-    a0 *= F_0_298631336; a1 *= F_2_053119869; a2 *= F_3_072711026; a3 *= F_1_501321110;
-    z1 *= -F_0_899976223; z2 *= -F_2_562915447; z3 *= -F_1_961570560; z4 *= -F_0_390180644;
-    z3 += z5; z4 += z5;
-    r.o0 = a0 + z1 + z3; r.o1 = a1 + z2 + z4; r.o2 = a2 + z2 + z3; r.o3 = a3 + z1 + z4;
-    return r;
-}
-
-// coef: dequantised coefficients in natural order; out: 8 rows of 8 samples, `stride` apart.  Columns / rows whose AC terms are all
-// zero take a shortcut that gives exactly what the full butterfly gives for them (dc << 2, resp. (ws0 + 16) >> 5).
-void idct_block(const int32_t coef[64], uint8_t* out, size_t stride) {
-    wide ws[64];
-    for (int c = 0; c < 8; ++c) {
-        if ((coef[8 + c] | coef[16 + c] | coef[24 + c] | coef[32 + c] | coef[40 + c] | coef[48 + c] | coef[56 + c]) == 0) {
-            const wide v = wide(coef[c]) * (1 << kPass1Bits);
-            ws[c] = ws[8 + c] = ws[16 + c] = ws[24 + c] = ws[32 + c] = ws[40 + c] = ws[48 + c] = ws[56 + c] = v;
-            continue;
-        }
-        const Butterfly b = idct_1d(coef[c], coef[8 + c], coef[16 + c], coef[24 + c], coef[32 + c], coef[40 + c], coef[48 + c], coef[56 + c]);
-        const int s = kConstBits - kPass1Bits;
-        ws[c] = descale(b.e0 + b.o3, s);       ws[56 + c] = descale(b.e0 - b.o3, s);
-        ws[8 + c] = descale(b.e1 + b.o2, s);   ws[48 + c] = descale(b.e1 - b.o2, s);
-        ws[16 + c] = descale(b.e2 + b.o1, s);  ws[40 + c] = descale(b.e2 - b.o1, s);
-        ws[24 + c] = descale(b.e3 + b.o0, s);  ws[32 + c] = descale(b.e3 - b.o0, s);
-    }
-    for (int r = 0; r < 8; ++r) {
-        const wide* w = ws + 8 * r;
-        uint8_t* o = out + r * stride;
-        if ((w[1] | w[2] | w[3] | w[4] | w[5] | w[6] | w[7]) == 0) {
-            memset(o, clamp_sample(descale(w[0], kPass1Bits + 3)), 8);
-            continue;
-        }
-        const Butterfly b = idct_1d(w[0], w[1], w[2], w[3], w[4], w[5], w[6], w[7]);
-        const int s = kConstBits + kPass1Bits + 3;
-        o[0] = clamp_sample(descale(b.e0 + b.o3, s));  o[7] = clamp_sample(descale(b.e0 - b.o3, s));
-        o[1] = clamp_sample(descale(b.e1 + b.o2, s));  o[6] = clamp_sample(descale(b.e1 - b.o2, s));
-        o[2] = clamp_sample(descale(b.e2 + b.o1, s));  o[5] = clamp_sample(descale(b.e2 - b.o1, s));
-        o[3] = clamp_sample(descale(b.e3 + b.o0, s));  o[4] = clamp_sample(descale(b.e3 - b.o0, s));
-    }
-}
+// ---- inverse DCT, accurate integer method: the 64-bit scalar transform is mdcj::idct_block (mdc_jpeg_entropy.cuh), shared with the
+// GPU decoder
+using mdcj::wide; using mdcj::kConstBits; using mdcj::kPass1Bits; using mdcj::descale; using mdcj::clamp_sample; using mdcj::idct_block;
+using mdcj::F_0_298631336; using mdcj::F_0_390180644; using mdcj::F_0_541196100; using mdcj::F_0_765366865; using mdcj::F_0_899976223;
+using mdcj::F_1_175875602; using mdcj::F_1_501321110; using mdcj::F_1_847759065; using mdcj::F_1_961570560; using mdcj::F_2_053119869;
+using mdcj::F_2_562915447; using mdcj::F_3_072711026;
 
 // ---- the same transform with AVX2: eight columns (pass 1) resp. eight rows (pass 2) per instruction, 32-bit lanes.  Dequantised
 // coefficients of a valid stream fit 16 bits, so no lane can overflow and the results equal the 64-bit scalar code bit for bit
@@ -355,14 +243,15 @@ inline int be16(const uint8_t* p) { return (p[0] << 8) | p[1]; }
 
 }  // namespace
 
-bool mdc_decode_jpeg_gray(const std::vector<uint8_t>& file, const std::string& name, mdc_gray_image* out) {
-    const uint8_t* d = file.data();
-    const size_t n = file.size();
+bool mdc_jpeg_parse_header(const uint8_t* d, size_t n, const std::string& name, mdc_jpeg_header* h) {
     if (n < 4 || d[0] != 0xff || d[1] != 0xd8) { mdc_set_error("%s: not a JPEG file", name.c_str()); return false; }
     uint16_t quant[4][64];
     bool quant_defined[4] = {false, false, false, false};
-    HuffTable dc[4], ac[4];
-    std::vector<Component> comps;
+    HuffTable* dc = h->dc;
+    HuffTable* ac = h->ac;
+    for (int t = 0; t < 4; ++t) dc[t].defined = ac[t].defined = false;
+    mdc_jpeg_component* comps = h->comp;
+    int ncomp = 0;
     int width = 0, height = 0, restart_interval = 0;
     bool have_frame = false;
     size_t pos = 2;
@@ -416,8 +305,9 @@ bool mdc_decode_jpeg_gray(const std::vector<uint8_t>& file, const std::string& n
             const int nc = seg[5];
             if ((nc != 1 && nc != 3) || seg_len < 6 + 3 * nc || width < 1 || height < 1) return fail("unsupported JPEG frame (components / size)");
             if (static_cast<long long>(width) * height > (1LL << 28)) return fail("JPEG frame larger than 2^28 pixels");
-            comps.resize(static_cast<size_t>(nc));
+            ncomp = nc;
             for (int c = 0; c < nc; ++c) {
+                comps[c] = mdc_jpeg_component();
                 comps[c].id = seg[6 + 3 * c];
                 comps[c].h = seg[7 + 3 * c] >> 4;
                 comps[c].v = seg[7 + 3 * c] & 15;
@@ -434,92 +324,131 @@ bool mdc_decode_jpeg_gray(const std::vector<uint8_t>& file, const std::string& n
             if (!have_frame) return fail("scan before frame header");
             if (seg_len < 1) return fail("bad scan header");
             const int ns = seg[0];
-            if (ns != static_cast<int>(comps.size()) || seg_len < 1 + 2 * ns + 3) return fail("non-interleaved multi-scan JPEG is not supported");
+            if (ns != ncomp || seg_len < 1 + 2 * ns + 3) return fail("non-interleaved multi-scan JPEG is not supported");
             for (int k = 0; k < ns; ++k) {
                 const int cid = seg[1 + 2 * k];
                 bool found = false;
-                for (size_t c = 0; c < comps.size(); ++c)
+                for (int c = 0; c < ncomp; ++c)
                     if (comps[c].id == cid) { comps[c].td = seg[2 + 2 * k] >> 4; comps[c].ta = seg[2 + 2 * k] & 15; found = true; }
                 if (!found) return fail("scan names an unknown component");
             }
             pos += static_cast<size_t>(len);
-            // ---- decode the scan
             int hmax = 1, vmax = 1;
-            for (size_t c = 0; c < comps.size(); ++c) { hmax = std::max(hmax, comps[c].h); vmax = std::max(vmax, comps[c].v); comps[c].pred = 0; }
-            const Component& Y = comps[0];
+            for (int c = 0; c < ncomp; ++c) { hmax = std::max(hmax, comps[c].h); vmax = std::max(vmax, comps[c].v); }
+            const mdc_jpeg_component& Y = comps[0];
             if (!quant_defined[Y.tq]) return fail("missing quantisation table");
-            for (size_t c = 0; c < comps.size(); ++c)
+            for (int c = 0; c < ncomp; ++c)
                 if (comps[c].td > 3 || comps[c].ta > 3 || !dc[comps[c].td].defined || !ac[comps[c].ta].defined) return fail("missing Huffman table");
-            const bool single = comps.size() == 1;
+            const bool single = ncomp == 1;
             // a single-component scan is not interleaved: its MCU is one block whatever the sampling factors say (T.81 A.2.2)
             const int mcu_w = single ? 8 : 8 * hmax, mcu_h = single ? 8 : 8 * vmax;
-            const int mcus_x = (width + mcu_w - 1) / mcu_w, mcus_y = (height + mcu_h - 1) / mcu_h;
-            const int yh = single ? 1 : Y.h, yv = single ? 1 : Y.v;
             // luminance plane padded to whole blocks; for subsampled colour files Y has h x v blocks per MCU at full resolution
             // only if Y carries the maximum factors (always the case for files written by libjpeg/OpenCV); otherwise Y itself
             // is subsampled and a grey read would need upsampling, which is not supported
             if (!single && (Y.h != hmax || Y.v != vmax)) return fail("JPEG with a subsampled luminance component is not supported");
-            const size_t pw = static_cast<size_t>(mcus_x) * yh * 8, ph = static_cast<size_t>(mcus_y) * yv * 8;
-            // per-thread scratch, reused from frame to frame: a fresh 2 MB vector per frame means mmap + page faults + munmap on
-            // every decode, and with dozens of decode threads those serialise on the process's address-space lock
-            // When the width is a whole number of blocks the padded plane is the image plus spare rows: decode straight into the
-            // result and cut the spare rows off afterwards (one 2 MB copy less per frame).
-            static thread_local std::vector<uint8_t> scratch_plane;
-            const bool in_place = pw == static_cast<size_t>(width);
-            std::vector<uint8_t>& plane = in_place ? out->px : scratch_plane;
-            plane.resize(pw * ph);      // every block of the padded plane is written by the loop below
-            BitReader br{d + pos, d + n};
-            alignas(32) int32_t coef[64] = {0};      // all zero between blocks: a block clears what it wrote
-            int32_t qzz[64];                         // luminance quantisation steps in zig-zag (= stream) order
-            for (int k = 0; k < 64; ++k) qzz[k] = quant[Y.tq][kZigZag[k]];
-            int until_restart = restart_interval;
-            for (int my = 0; my < mcus_y; ++my)
-                for (int mx = 0; mx < mcus_x; ++mx) {
-                    if (restart_interval && until_restart == 0) {
-                        // byte-align, expect RSTn, reset predictors
-                        const uint8_t* q = br.p;
-                        while (q + 1 < br.end && !(q[0] == 0xff && q[1] >= 0xd0 && q[1] <= 0xd7)) ++q;
-                        if (q + 1 >= br.end) return fail("missing restart marker");
-                        br.p = q + 2;
-                        br.reset();
-                        for (size_t c = 0; c < comps.size(); ++c) comps[c].pred = 0;
-                        until_restart = restart_interval;
-                    }
-                    for (size_t c = 0; c < comps.size(); ++c) {
-                        Component& comp = comps[c];
-                        const int bh = single ? 1 : comp.h, bv = single ? 1 : comp.v;
-                        for (int by = 0; by < bv; ++by)
-                            for (int bx = 0; bx < bh; ++bx) {
-                                const int rc = c == 0 ? decode_block<true>(br, dc[comp.td], ac[comp.ta], comp.pred, coef, qzz)
-                                                      : decode_block<false>(br, dc[comp.td], ac[comp.ta], comp.pred, nullptr, qzz);
-                                if (rc < 0) return fail(rc == kBlockBadDc ? "corrupt JPEG data (DC)" : rc == kBlockBadAc ? "corrupt JPEG data (AC)" : "corrupt JPEG data (run past the block)");
-                                const bool any_ac = rc != 0;
-                                if (c == 0) {
-                                    const size_t x0 = (static_cast<size_t>(mx) * yh + bx) * 8, y0 = (static_cast<size_t>(my) * yv + by) * 8;
-                                    uint8_t* dst = plane.data() + y0 * pw + x0;
-                                    if (!any_ac) {
-                                        idct_dc_only(coef[0], dst, pw);
-                                        coef[0] = 0;
-                                    } else {
-#ifdef MDC_JPEG_AVX2
-                                        if (cpu_has_avx2) idct_block_avx2(coef, dst, pw);
-                                        else
-#endif
-                                            idct_block(coef, dst, pw);
-                                        memset(coef, 0, sizeof coef);
-                                    }
-                                }
-                            }
-                    }
-                    if (restart_interval) --until_restart;
-                }
-            out->rows = height; out->cols = width; out->depth = 8;
-            out->px.resize(static_cast<size_t>(width) * height);
-            if (!in_place)
-                for (int y = 0; y < height; ++y) memcpy(out->px.data() + static_cast<size_t>(y) * width, plane.data() + static_cast<size_t>(y) * pw, static_cast<size_t>(width));
+            h->width = width; h->height = height; h->ncomp = ncomp; h->restart_interval = restart_interval;
+            h->mcus_x = (width + mcu_w - 1) / mcu_w;
+            h->mcus_y = (height + mcu_h - 1) / mcu_h;
+            h->yh = single ? 1 : Y.h;
+            h->yv = single ? 1 : Y.v;
+            for (int k = 0; k < 64; ++k) h->qzz[k] = quant[Y.tq][kZigZag[k]];
+            h->scan_begin = pos;
             return true;
         }
         pos += static_cast<size_t>(len);
     }
     return fail("JPEG without image data");
+}
+
+// The host decoder's restart walk (mdc_decode_jpeg_gray): after an interval it searches for FF D0..D7 from the byte its reader
+// stopped at.  That reader never passes the first marker after the interval's start, and no FF D0..D7 lies in front of that marker
+// (an FF inside the interval is stuffed, FF 00), so searching from the interval's start finds the same marker.
+bool mdc_jpeg_split_segments(const uint8_t* d, size_t n, const mdc_jpeg_header& h, std::vector<mdc_jpeg_segment>* segs) {
+    segs->clear();
+    const int total = h.mcus_x * h.mcus_y;
+    const int per = h.restart_interval ? h.restart_interval : total;
+    size_t begin = h.scan_begin;
+    for (int first = 0; first < total; first += per) {
+        if (first > 0) {
+            size_t q = begin;
+            while (q + 1 < n && !(d[q] == 0xff && d[q + 1] >= 0xd0 && d[q + 1] <= 0xd7)) ++q;
+            if (q + 1 >= n) return false;
+            begin = q + 2;
+        }
+        size_t end = begin;                   // the first marker: an FF not followed by 00 (an FF as the last byte counts as one)
+        while (end < n && !(d[end] == 0xff && !(end + 1 < n && d[end + 1] == 0x00))) end += d[end] == 0xff ? 2 : 1;
+        segs->push_back(mdc_jpeg_segment{begin, end, first, std::min(per, total - first)});
+    }
+    return true;
+}
+
+bool mdc_decode_jpeg_gray(const std::vector<uint8_t>& file, const std::string& name, mdc_gray_image* out) {
+    const uint8_t* d = file.data();
+    const size_t n = file.size();
+    static thread_local mdc_jpeg_header hdr;      // 46 KB of Huffman tables: not on the decode threads' stacks
+    if (!mdc_jpeg_parse_header(d, n, name, &hdr)) return false;
+    const mdc_jpeg_header& h = hdr;
+    auto fail = [&](const char* what) { mdc_set_error("%s: %s", name.c_str(), what); return false; };
+    const int width = h.width, height = h.height, restart_interval = h.restart_interval;
+    const int mcus_x = h.mcus_x, mcus_y = h.mcus_y, yh = h.yh, yv = h.yv;
+    const bool single = h.ncomp == 1;
+    int pred[3] = {0, 0, 0};
+    const size_t pw = static_cast<size_t>(mcus_x) * yh * 8, ph = static_cast<size_t>(mcus_y) * yv * 8;
+    // per-thread scratch, reused from frame to frame: a fresh 2 MB vector per frame means mmap + page faults + munmap on
+    // every decode, and with dozens of decode threads those serialise on the process's address-space lock
+    // When the width is a whole number of blocks the padded plane is the image plus spare rows: decode straight into the
+    // result and cut the spare rows off afterwards (one 2 MB copy less per frame).
+    static thread_local std::vector<uint8_t> scratch_plane;
+    const bool in_place = pw == static_cast<size_t>(width);
+    std::vector<uint8_t>& plane = in_place ? out->px : scratch_plane;
+    plane.resize(pw * ph);      // every block of the padded plane is written by the loop below
+    BitReader br{d + h.scan_begin, d + n};
+    alignas(32) int32_t coef[64] = {0};      // all zero between blocks: a block clears what it wrote
+    const int32_t* qzz = h.qzz;              // luminance quantisation steps in zig-zag (= stream) order
+    int until_restart = restart_interval;
+    for (int my = 0; my < mcus_y; ++my)
+        for (int mx = 0; mx < mcus_x; ++mx) {
+            if (restart_interval && until_restart == 0) {
+                // byte-align, expect RSTn, reset predictors
+                const uint8_t* q = br.p;
+                while (q + 1 < br.end && !(q[0] == 0xff && q[1] >= 0xd0 && q[1] <= 0xd7)) ++q;
+                if (q + 1 >= br.end) return fail("missing restart marker");
+                br.p = q + 2;
+                br.reset();
+                pred[0] = pred[1] = pred[2] = 0;
+                until_restart = restart_interval;
+            }
+            for (int c = 0; c < h.ncomp; ++c) {
+                const mdc_jpeg_component& comp = h.comp[c];
+                const int bh = single ? 1 : comp.h, bv = single ? 1 : comp.v;
+                for (int by = 0; by < bv; ++by)
+                    for (int bx = 0; bx < bh; ++bx) {
+                        const int rc = c == 0 ? decode_block<true>(br, h.dc[comp.td], h.ac[comp.ta], pred[c], coef, qzz)
+                                              : decode_block<false>(br, h.dc[comp.td], h.ac[comp.ta], pred[c], nullptr, qzz);
+                        if (rc < 0) return fail(rc == kBlockBadDc ? "corrupt JPEG data (DC)" : rc == kBlockBadAc ? "corrupt JPEG data (AC)" : "corrupt JPEG data (run past the block)");
+                        const bool any_ac = rc != 0;
+                        if (c == 0) {
+                            const size_t x0 = (static_cast<size_t>(mx) * yh + bx) * 8, y0 = (static_cast<size_t>(my) * yv + by) * 8;
+                            uint8_t* dst = plane.data() + y0 * pw + x0;
+                            if (!any_ac) {
+                                idct_dc_only(coef[0], dst, pw);
+                                coef[0] = 0;
+                            } else {
+#ifdef MDC_JPEG_AVX2
+                                if (cpu_has_avx2) idct_block_avx2(coef, dst, pw);
+                                else
+#endif
+                                    idct_block(coef, dst, pw);
+                                memset(coef, 0, sizeof coef);
+                            }
+                        }
+                    }
+            }
+            if (restart_interval) --until_restart;
+        }
+    out->rows = height; out->cols = width; out->depth = 8;
+    out->px.resize(static_cast<size_t>(width) * height);
+    if (!in_place)
+        for (int y = 0; y < height; ++y) memcpy(out->px.data() + static_cast<size_t>(y) * width, plane.data() + static_cast<size_t>(y) * pw, static_cast<size_t>(width));
+    return true;
 }

@@ -64,6 +64,7 @@ struct mdc_seq {
     mutable void* stage[2] = {nullptr, nullptr};
     mutable size_t stage_bytes = 0;
     mutable std::mutex feed_mutex;
+    mutable mdc_seq_feed_stage device_stage;      // the same for mdc_seq_prepare_device (mdc_jpeg_gpu.cu)
 };
 
 namespace {
@@ -210,6 +211,18 @@ bool read_gray8(const mdc_seq* s, int id, std::vector<uint8_t>* px, int* w, int*
 
 }  // namespace
 
+bool mdc_seq_read_file(const mdc_seq* s, int id, std::vector<uint8_t>* file) {
+    try {
+        if (s->zipped) return read_zip_entry(s, s->entries[static_cast<size_t>(id)], file);
+        return mdc_read_file(s->files[static_cast<size_t>(id)], file);
+    } catch (const std::exception& e) {
+        mdc_set_error("%s: cannot read (%s)", s->files[static_cast<size_t>(id)].c_str(), e.what());
+        return false;
+    }
+}
+std::mutex& mdc_seq_feed_mutex(const mdc_seq* s) { return s->feed_mutex; }
+mdc_seq_feed_stage* mdc_seq_device_stage(const mdc_seq* s) { return &s->device_stage; }
+
 extern "C" int mdc_seq_open(const char* folder, mdc_seq** out) {
     if (!folder || !out) { mdc_set_error("mdc_seq_open: bad argument"); return MDC_ERR_INVALID_ARG; }
     *out = nullptr;
@@ -245,6 +258,7 @@ extern "C" int mdc_seq_open(const char* folder, mdc_seq** out) {
 extern "C" void mdc_seq_close(mdc_seq* s) {
     if (!s) return;
     for (int b = 0; b < 2; ++b) if (s->stage[b]) mdc_host_free(s->stage[b]);
+    for (int b = 0; b < 2; ++b) if (s->device_stage.pinned[b]) mdc_host_free(s->device_stage.pinned[b]);
     if (s->zip_fd >= 0) close(s->zip_fd);
     delete s;
 }
@@ -275,7 +289,7 @@ extern "C" int mdc_seq_read_gray8(const mdc_seq* s, int id, uint8_t* out, size_t
 
 // threads = 0: as many decode threads as the process may keep busy — the CPUs it is allowed to run on, capped by the container's
 // CPU-time quota (cgroup v2 cpu.max) where there is one: more busy threads than the quota only get throttled
-static int default_decode_threads() {
+int mdc_seq_default_threads() {
     int n = static_cast<int>(std::max(1u, std::thread::hardware_concurrency()));
     cpu_set_t set;
     if (sched_getaffinity(0, sizeof set, &set) == 0) n = std::max(1, std::min(n, CPU_COUNT(&set)));
@@ -317,7 +331,7 @@ extern "C" int mdc_seq_prepare(mdc_ctx* c, const mdc_seq* s, int first, int coun
         }
     }
     if (count == 0) return MDC_OK;
-    if (threads < 1) threads = default_decode_threads();
+    if (threads < 1) threads = mdc_seq_default_threads();
     // a chunk is what the GPU side takes at a time: two frames per decode thread (handed out dynamically, so a slow frame or a
     // descheduled thread does not hold the chunk up), small enough that the un-overlapped head (first decode) and tail (last
     // H2D / K1 / D2H) of a call stay short
