@@ -236,6 +236,20 @@ int mdc_seq_prepare(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned
  * are complete, and nothing from its chunk on is written.  Returns when the work is done on the device. */
 int mdc_seq_prepare_device(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned flags, float* const* d_out_levels, int levels,
                            int threads, mdc_stream stream);
+/* getImageRaw_internal(ids[k]) for k < n into DEVICE memory: frame k -> d_out + k*h*row_pitch (row_pitch >= w; a multiple of 16 keeps
+ * mdc_prepare_batch_pitched on its TMA loader).  ids may be in any order and may repeat.  The same device feed as mdc_seq_prepare_device
+ * (`threads` host threads, 0 = the default count; chunks of min(512, max(16, 32 * threads)) frames; JPEG frames decoded on the GPU,
+ * PNG / PGM frames on the host; `stream` as for mdc_prepare_batch), without the fused kernel.  Per frame, the outcome of
+ * mdc_seq_read_gray8(s, ids[k], ...): status_host[k] (n ints, may be NULL) is MDC_OK if the frame reads and is w x h, and its rows
+ * then hold the host reader's bytes; MDC_ERR_FORMAT if the host reader fails on it; MDC_ERR_INVALID_ARG if it reads at another size.
+ * sizes_host (2*n ints: w h per frame, may be NULL) gets the size the host reader reports, or 0 0 if it fails.  Rows of a frame that
+ * is not MDC_OK, and the padding bytes of every row, are left untouched; the frames around a failed one are still written.
+ * Returns MDC_ERR_INVALID_ARG before anything is read for n < 0, a NULL c, s, ids or d_out with n > 0, an id outside the sequence,
+ * w or h < 1 or row_pitch < w (none of which needs a device; n = 0 is a no-op); otherwise MDC_OK if every frame is MDC_OK,
+ * MDC_ERR_FORMAT with the first such frame's message if not, MDC_ERR_CUDA on a runtime failure.  Returns when the frames are on
+ * the device. */
+int mdc_seq_read_gray8_device(mdc_ctx* c, const mdc_seq* s, const int* ids, int n, int w, int h, uint8_t* d_out, size_t row_pitch,
+                              int* status_host, int* sizes_host, int threads, mdc_stream stream);
 /* Baseline JPEGs in HOST memory (files[i], sizes[i] bytes) -> 8-bit grey planes on the device, the same bytes as mdc_seq_read_gray8
  * (the host decoder): d_out is [n][h][row_pitch] (row_pitch >= w; a multiple of 16 keeps mdc_prepare_batch_pitched on its TMA
  * loader).  Headers are parsed on the host; a frame the parser rejects, or one that is not w x h, is never uploaded, and the frames

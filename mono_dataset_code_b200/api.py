@@ -581,6 +581,29 @@ class Sequence:
                                          len(out), threads, stream), "mdc_seq_prepare_device")
         return out
 
+    def read_gray8_device(self, ctx: "Context", ids, w: int, h: int, row_pitch: int | None = None, threads: int = 0, out=None):
+        """getImageRaw_internal(id) for every id (any order, repeats allowed), decoded into device memory (mdc_seq_read_gray8_device) ->
+        (uint8 CUDA tensor [n, h, row_pitch] on the context's device, status int32 [n], sizes int32 [n, 2]).  Per frame, as
+        mdc_seq_read_gray8: status 0 = read at w x h; 3 = MDC_ERR_FORMAT, it cannot be read; 1 = MDC_ERR_INVALID_ARG, it reads at
+        another size.  sizes holds (w, h) as the host reader reports them, (0, 0) if it cannot read the frame.  Rows of a frame that
+        is not read, and the padding of every row, keep what `out` held.  row_pitch defaults to w rounded up to 16 bytes.  Runs on
+        torch's current stream; bad arguments and runtime failures raise MdcError."""
+        import torch
+        ids = np.ascontiguousarray(ids, dtype=np.int32).reshape(-1)
+        n = ids.size
+        pitch = row_pitch if row_pitch is not None else (w + 15) // 16 * 16
+        if out is None:
+            out = torch.zeros((n, h, pitch), dtype=torch.uint8, device=f"cuda:{ctx.device}")
+        elif out.dtype != torch.uint8 or not out.is_cuda or not out.is_contiguous() or tuple(out.shape) != (n, h, pitch):
+            raise ValueError(f"out must be a contiguous uint8 CUDA tensor of shape {(n, h, pitch)}")
+        status = np.zeros(n, np.int32)
+        sizes = np.zeros((n, 2), np.int32)
+        rc = lib.mdc_seq_read_gray8_device(ctx._h, self._h, ids.ctypes.data, n, w, h, C.c_void_p(out.data_ptr()), pitch, status.ctypes.data,
+                                           sizes.ctypes.data, threads, Context._stream(out))
+        if rc not in (0, 3):
+            check(rc, "mdc_seq_read_gray8_device")
+        return out, status, sizes
+
 
 class FramePreparer:
     """The getImage composition of DatasetReader (BenchmarkDatasetReader.h:188-243) over frames that are already decoded

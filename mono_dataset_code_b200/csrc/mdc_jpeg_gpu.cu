@@ -6,7 +6,9 @@
 //   J2     inverse DCT: eight threads per 8x8 block (a column each, then a row each), exactly mdcj::idct_block; cropped samples
 //          into a u8 batch [n][h][row_pitch]
 //   errors per frame in a status word (the first failing segment and its kind), never a trap
-// mdc_jpeg_decode_device decodes host buffers; mdc_seq_prepare_device feeds a sequence through H2D -> J1 -> J2 -> K1 chunk by chunk.
+// mdc_jpeg_decode_device decodes host buffers.  One device feed (run_device_feed) reads a sequence's frames on host threads and sends
+// them H2D -> J1 -> J2 chunk by chunk: mdc_seq_prepare_device runs K1 on each chunk, mdc_seq_read_gray8_device leaves the raw frames in
+// the caller's rows.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -15,6 +17,7 @@
 #include <cstdio>
 #include <cstring>
 #include <exception>
+#include <functional>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -340,10 +343,243 @@ struct FeedFrame {
     std::unique_ptr<mdc_jpeg_header> hdr;      // JPEG: the parsed header
     std::vector<mdc_jpeg_segment> segs;
     bool jpeg = false, complete = true;
+    int status = MDC_OK;                       // MDC_OK: goes to the GPU; MDC_ERR_FORMAT: the host reader fails on it; MDC_ERR_INVALID_ARG: it reads, at another size
+    int w = 0, h = 0;                          // the size the host reader reports (0 0 if it fails)
+    std::string msg;                           // why the frame is not MDC_OK
 };
 
 // the frames a chunk of the device feed holds: more frames decode at once in J1, which keeps more of the GPU busy
 int device_feed_chunk(int threads) { return std::min(512, std::max(16, 32 * threads)); }
+
+// Reads frame `id` of `s` into `ff`: the file, then a JPEG's header and restart split (its entropy decoding is the GPU's), or a PNG /
+// PGM decoded to 8 bits.  The outcome is the one mdc_seq_read_gray8 would have, with frames of another size than w x h marked.
+void read_feed_frame(const mdc_seq* s, int id, int w, int h, FeedFrame& ff, mdc_gray_image& img) {
+    const std::string name = mdc_seq_name(s, id);
+    ff.jpeg = false;
+    ff.status = MDC_ERR_FORMAT;
+    ff.w = ff.h = 0;
+    ff.msg.clear();
+    int fw = 0, fh = 0;
+    try {
+        if (!mdc_seq_read_file(s, id, &ff.file)) { ff.msg = mdc_last_error(); return; }
+        if (ff.file.size() >= 2 && ff.file[0] == 0xff && ff.file[1] == 0xd8) {
+            if (!ff.hdr) ff.hdr.reset(new mdc_jpeg_header);
+            if (!mdc_jpeg_parse_header(ff.file.data(), ff.file.size(), name, ff.hdr.get())) { ff.msg = mdc_last_error(); return; }
+            fw = ff.hdr->width; fh = ff.hdr->height;
+            if (fw != w || fh != h) {         // not decoded on the GPU: whether the host decoder accepts it decides its status
+                if (!mdc_decode_gray_image(ff.file, name, &img)) { ff.msg = mdc_last_error(); return; }
+            } else {
+                ff.jpeg = true;
+                ff.complete = mdc_jpeg_split_segments(ff.file.data(), ff.file.size(), *ff.hdr, &ff.segs);
+            }
+        } else {
+            if (!mdc_decode_gray_image(ff.file, name, &img)) { ff.msg = mdc_last_error(); return; }
+            fw = img.cols; fh = img.rows;
+            const size_t npx = static_cast<size_t>(fw) * fh;
+            if (img.depth == 8) {
+                ff.px.swap(img.px);
+            } else {                          // 16-bit: the high byte, as mdc_seq_read_gray8
+                ff.px.resize(npx);
+                const uint16_t* src = reinterpret_cast<const uint16_t*>(img.px.data());
+                for (size_t p = 0; p < npx; ++p) ff.px[p] = static_cast<uint8_t>(src[p] >> 8);
+            }
+        }
+    } catch (const std::exception& e) {
+        ff.jpeg = false;
+        ff.msg = name + ": cannot read (" + e.what() + ")";
+        return;
+    }
+    ff.w = fw; ff.h = fh;
+    ff.status = MDC_OK;
+    if (fw != w || fh != h) {                 // BenchmarkDatasetReader.h:194-199
+        char msg[256];
+        snprintf(msg, sizeof msg, "expected image dimensions %d x %d; found %d x %d (image %s)", w, h, fw, fh, name.c_str());
+        ff.jpeg = false;
+        ff.status = MDC_ERR_INVALID_ARG;
+        ff.msg = msg;
+    }
+}
+
+// Chunk [f0, f0 + n) of a device feed after J1 / J2, per frame: the status and size mdc_seq_read_gray8 would give (FeedFrame), its
+// message, and where J2 wrote the frames that are MDC_OK ([n][h][pitch]).
+struct FeedChunk {
+    int f0 = 0, n = 0;
+    uint8_t* frames = nullptr;
+    std::vector<int> status, sizes;            // sizes: w h per frame
+    std::vector<std::string> msg;
+};
+
+// The device feed behind mdc_seq_prepare_device and mdc_seq_read_gray8_device: frames ids[0 .. count) of `s`, which the reader
+// expects to be w x h, in chunks of device_feed_chunk(threads).  `threads` host threads read the files, parse the JPEG headers,
+// split the scans and decode PNG / PGM frames for chunk k+1 while the main thread packs chunk k into the sequence's pinned staging
+// and sends it H2D -> J1 -> J2 on `st`.  J2 writes chunk k's frames to d_out + f0 * h * pitch (their slots of the caller's rows) or,
+// with d_out NULL, to a scratch buffer of the chunk's slot.  Once a chunk's status words are back, consume(chunk) runs (it may
+// enqueue more work on `st` that reads chunk.frames); the feed stops at the first consume that does not return MDC_OK and returns
+// that code.  Frames that fail are never written.  Returns after `st` has drained.
+int run_device_feed(const mdc_seq* s, const int* ids, int count, int w, int h, int threads, uint8_t* d_out, size_t pitch, cudaStream_t st,
+                    const std::function<int(const FeedChunk&)>& consume, const char* who) {
+    const int chunk = device_feed_chunk(threads);
+    std::lock_guard<std::mutex> feed_lock(mdc_seq_feed_mutex(s));
+    mdc_seq_feed_stage* stage = mdc_seq_device_stage(s);
+
+    const int n_chunks = (count + chunk - 1) / chunk;
+    const int workers = std::min(threads, std::min(count, chunk));
+    std::vector<FeedFrame> frames[2];
+    for (int b = 0; b < 2; ++b) frames[b].resize(static_cast<size_t>(std::min(chunk, count)));
+    std::mutex mu;
+    std::condition_variable cv;
+    std::vector<int> decoded(static_cast<size_t>(n_chunks), 0);
+    std::vector<std::atomic<int>> next_frame(static_cast<size_t>(n_chunks));
+    for (auto& a : next_frame) a.store(0, std::memory_order_relaxed);
+    int released = 1;                 // chunks whose frame slots may be written: 0 .. released
+    bool abort = false;
+    auto worker = [&](int) {
+        mdc_gray_image img;
+        for (int k = 0; k < n_chunks; ++k) {
+            {
+                std::unique_lock<std::mutex> lk(mu);
+                cv.wait(lk, [&] { return abort || k <= released; });
+                if (abort) return;
+            }
+            const int f0 = k * chunk, n = std::min(chunk, count - f0);
+            for (int i; (i = next_frame[static_cast<size_t>(k)].fetch_add(1, std::memory_order_relaxed)) < n;)
+                read_feed_frame(s, ids[f0 + i], w, h, frames[k & 1][static_cast<size_t>(i)], img);
+            std::lock_guard<std::mutex> lk(mu);
+            ++decoded[static_cast<size_t>(k)];
+            cv.notify_all();
+        }
+    };
+    std::vector<std::thread> pool;
+    try {
+        for (int t = 0; t < workers; ++t) pool.emplace_back(worker, t);
+    } catch (const std::exception& e) {
+        { std::lock_guard<std::mutex> lk(mu); abort = true; }
+        cv.notify_all();
+        for (auto& th : pool) th.join();
+        mdc_set_error("%s: cannot start decode threads (%s)", who, e.what());
+        return MDC_ERR_IO;
+    }
+
+    HostBatch batch[2];
+    FeedChunk done[2];                // the host side of each slot's chunk, kept after its frame slots are handed to chunk k + 2
+    DevSlot dev[2];
+    cudaEvent_t ev_status[2] = {nullptr, nullptr}, ev_done[2] = {nullptr, nullptr};
+    uint32_t* status_pinned[2] = {nullptr, nullptr};
+    int rc = MDC_OK;
+    for (int b = 0; b < 2 && rc == MDC_OK; ++b)
+        if (cudaEventCreateWithFlags(&ev_status[b], cudaEventDisableTiming) != cudaSuccess ||
+            cudaEventCreateWithFlags(&ev_done[b], cudaEventDisableTiming) != cudaSuccess ||
+            cudaEventRecord(ev_done[b], st) != cudaSuccess) {
+            mdc_set_error("%s: cannot create events", who);
+            rc = MDC_ERR_CUDA;
+        }
+    // chunk k: pack into pinned staging, then H2D -> J1 -> J2 (-> status D2H) on the stream
+    auto submit = [&](int k) -> int {
+        const int b = k & 1, f0 = k * chunk, n = std::min(chunk, count - f0);
+        HostBatch& hb = batch[b];
+        hb = HostBatch();
+        FeedChunk& fc = done[b];
+        fc.f0 = f0;
+        fc.n = n;
+        fc.status.resize(static_cast<size_t>(n));
+        fc.sizes.resize(2 * static_cast<size_t>(n));
+        fc.msg.resize(static_cast<size_t>(n));
+        std::vector<size_t> at(static_cast<size_t>(n));
+        for (int i = 0; i < n; ++i) {
+            FeedFrame& ff = frames[b][static_cast<size_t>(i)];
+            fc.status[static_cast<size_t>(i)] = ff.status;
+            fc.sizes[2 * static_cast<size_t>(i)] = ff.w;
+            fc.sizes[2 * static_cast<size_t>(i) + 1] = ff.h;
+            fc.msg[static_cast<size_t>(i)].swap(ff.msg);
+            at[static_cast<size_t>(i)] = hb.bytes;
+            if (ff.status != MDC_OK) {
+                hb.add_skipped();
+            } else if (ff.jpeg) {
+                hb.add_jpeg(*ff.hdr, ff.segs, ff.complete, mdc_seq_name(s, ids[f0 + i]), hb.bytes);
+                hb.bytes += ff.segs.empty() ? 0 : ff.segs.back().end - ff.segs.front().begin;
+            } else {
+                hb.add_raw(hb.bytes);
+                hb.bytes += ff.px.size();
+            }
+        }
+        const size_t meta = hb.meta_bytes(), need = meta + HostBatch::align(hb.bytes) + sizeof(uint32_t) * static_cast<size_t>(n);
+        // the slot's previous chunk (k - 2) has left the staging buffer and the device buffers behind
+        CU_CHECK(cudaEventSynchronize(ev_done[b]));
+        if (stage->bytes[b] < need) {
+            if (stage->pinned[b]) mdc_host_free(stage->pinned[b]);
+            stage->pinned[b] = nullptr;
+            stage->bytes[b] = 0;
+            if (mdc_host_alloc(&stage->pinned[b], need + need / 8) != MDC_OK) return MDC_ERR_CUDA;
+            stage->bytes[b] = need + need / 8;
+        }
+        int r = prepare_slot(hb, dev[b]);
+        if (r == MDC_OK && !d_out) r = grow(&dev[b].u8, &dev[b].u8_cap, static_cast<size_t>(chunk) * h * pitch);
+        if (r != MDC_OK) return r;
+        uint8_t* pin = static_cast<uint8_t*>(stage->pinned[b]);
+        hb.write_meta(pin, dev[b].meta);
+        for (int i = 0; i < n; ++i) {
+            const FeedFrame& ff = frames[b][static_cast<size_t>(i)];
+            uint8_t* dst = pin + meta + at[static_cast<size_t>(i)];
+            if (ff.status != MDC_OK) continue;
+            if (ff.jpeg && !ff.segs.empty()) memcpy(dst, ff.file.data() + ff.segs.front().begin, ff.segs.back().end - ff.segs.front().begin);
+            else if (!ff.jpeg) memcpy(dst, ff.px.data(), ff.px.size());
+        }
+        fc.frames = d_out ? d_out + static_cast<size_t>(f0) * h * pitch : dev[b].u8;
+        status_pinned[b] = reinterpret_cast<uint32_t*>(pin + meta + HostBatch::align(hb.bytes));
+        r = enqueue_batch(hb, dev[b], pin, pin + meta, w, h, fc.frames, pitch, status_pinned[b], st);
+        if (r != MDC_OK) return r;
+        CU_CHECK(cudaEventRecord(ev_status[b], st));
+        return MDC_OK;
+    };
+    // chunk k after J1 / J2: the GPU's verdict joins the host's, then the consumer
+    auto finish = [&](int k) -> int {
+        const int b = k & 1;
+        FeedChunk& fc = done[b];
+        CU_CHECK(cudaEventSynchronize(ev_status[b]));
+        for (int i = 0; i < fc.n; ++i) {
+            if (fc.status[static_cast<size_t>(i)] != MDC_OK) continue;
+            std::string m;
+            if (status_pinned[b][i] != kStatusOk) m = std::string(mdc_seq_name(s, ids[fc.f0 + i])) + ": " + kind_message(status_pinned[b][i]);
+            else m = batch[b].incomplete_msg[static_cast<size_t>(i)];
+            if (m.empty()) continue;
+            fc.status[static_cast<size_t>(i)] = MDC_ERR_FORMAT;
+            fc.sizes[2 * static_cast<size_t>(i)] = fc.sizes[2 * static_cast<size_t>(i) + 1] = 0;
+            fc.msg[static_cast<size_t>(i)] = m;
+        }
+        const int r = consume(fc);
+        if (r != MDC_OK) return r;
+        CU_CHECK(cudaEventRecord(ev_done[b], st));
+        return MDC_OK;
+    };
+    for (int k = 0; k < n_chunks && rc == MDC_OK; ++k) {
+        {
+            std::unique_lock<std::mutex> lk(mu);
+            cv.wait(lk, [&] { return decoded[static_cast<size_t>(k)] == workers; });
+        }
+        rc = submit(k);
+        {
+            std::lock_guard<std::mutex> lk(mu);
+            released = k + 2;             // frames[k & 1] is packed: chunk k + 2 may be read into it
+        }
+        cv.notify_all();
+        if (rc == MDC_OK && k > 0) rc = finish(k - 1);          // overlaps chunk k's J1 / J2 on the GPU
+        if (rc == MDC_OK && k == n_chunks - 1) rc = finish(k);
+    }
+    {
+        std::lock_guard<std::mutex> lk(mu);
+        abort = true;
+    }
+    cv.notify_all();
+    for (auto& th : pool) th.join();
+    const cudaError_t drained = cudaStreamSynchronize(st);
+    if (rc == MDC_OK && drained != cudaSuccess) { mdc_set_error("%s: %s", who, cudaGetErrorString(drained)); rc = MDC_ERR_CUDA; }
+    for (int b = 0; b < 2; ++b) {
+        dev[b].release();
+        if (ev_status[b]) cudaEventDestroy(ev_status[b]);
+        if (ev_done[b]) cudaEventDestroy(ev_done[b]);
+    }
+    return rc;
+}
 
 }  // namespace
 
@@ -377,195 +613,57 @@ extern "C" int mdc_seq_prepare_device(mdc_ctx* c, const mdc_seq* s, int first, i
     if (threads < 1) threads = mdc_seq_default_threads();
     CU_CHECK(cudaSetDevice(mdc_ctx_device_ordinal(c)));
     cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : static_cast<cudaStream_t>(mdc_ctx_stream_handle(c));
-    const int chunk = device_feed_chunk(threads);
     // rows padded to 16 bytes keep K1 on its TMA loader; padded rows exist in rectifying mode only (mdc_prepare_batch_pitched)
     const size_t pitch = rectify ? (static_cast<size_t>(in_w) + 15) / 16 * 16 : static_cast<size_t>(in_w);
-    std::lock_guard<std::mutex> feed_lock(mdc_seq_feed_mutex(s));
-    mdc_seq_feed_stage* stage = mdc_seq_device_stage(s);
-
-    const int n_chunks = (count + chunk - 1) / chunk;
-    const int workers = std::min(threads, std::min(count, chunk));
-    std::vector<FeedFrame> frames[2];
-    for (int b = 0; b < 2; ++b) frames[b].resize(static_cast<size_t>(std::min(chunk, count)));
-    std::mutex mu;
-    std::condition_variable cv;
-    std::vector<int> decoded(static_cast<size_t>(n_chunks), 0);
-    std::vector<std::atomic<int>> next_frame(static_cast<size_t>(n_chunks));
-    for (auto& a : next_frame) a.store(0, std::memory_order_relaxed);
-    int released = 1;                 // chunks whose frame slots may be written: 0 .. released
-    bool abort = false;
-    std::vector<std::string> chunk_error(static_cast<size_t>(n_chunks));
-    // Workers: read the file, parse a JPEG's header and split its scan (the entropy decoding is the GPU's), decode other formats.
-    auto worker = [&](int) {
-        mdc_gray_image img;
-        for (int k = 0; k < n_chunks; ++k) {
-            {
-                std::unique_lock<std::mutex> lk(mu);
-                cv.wait(lk, [&] { return abort || k <= released; });
-                if (abort) return;
-            }
-            const int f0 = k * chunk, n = std::min(chunk, count - f0);
-            std::string err;
-            for (int i; err.empty() && (i = next_frame[static_cast<size_t>(k)].fetch_add(1, std::memory_order_relaxed)) < n;) {
-                const int id = first + f0 + i;
-                const std::string name = mdc_seq_name(s, id);
-                FeedFrame& ff = frames[k & 1][static_cast<size_t>(i)];
-                int w = 0, h = 0;
-                try {
-                    ff.jpeg = false;
-                    if (!mdc_seq_read_file(s, id, &ff.file)) { err = mdc_last_error(); break; }
-                    if (ff.file.size() >= 2 && ff.file[0] == 0xff && ff.file[1] == 0xd8) {
-                        if (!ff.hdr) ff.hdr.reset(new mdc_jpeg_header);
-                        if (!mdc_jpeg_parse_header(ff.file.data(), ff.file.size(), name, ff.hdr.get())) { err = mdc_last_error(); break; }
-                        w = ff.hdr->width; h = ff.hdr->height;
-                        ff.jpeg = true;
-                        ff.complete = mdc_jpeg_split_segments(ff.file.data(), ff.file.size(), *ff.hdr, &ff.segs);
-                    } else {
-                        if (!mdc_decode_gray_image(ff.file, name, &img)) { err = mdc_last_error(); break; }
-                        w = img.cols; h = img.rows;
-                        const size_t npx = static_cast<size_t>(w) * h;
-                        if (img.depth == 8) {
-                            ff.px.swap(img.px);
-                        } else {                // 16-bit: the high byte, as mdc_seq_read_gray8
-                            ff.px.resize(npx);
-                            const uint16_t* src = reinterpret_cast<const uint16_t*>(img.px.data());
-                            for (size_t p = 0; p < npx; ++p) ff.px[p] = static_cast<uint8_t>(src[p] >> 8);
-                        }
-                    }
-                } catch (const std::exception& e) {
-                    err = name + ": cannot read (" + e.what() + ")";
-                    break;
-                }
-                if (w != in_w || h != in_h) {      // BenchmarkDatasetReader.h:194-199
-                    char msg[256];
-                    snprintf(msg, sizeof msg, "expected image dimensions %d x %d; found %d x %d (image %s)", in_w, in_h, w, h, name.c_str());
-                    err = msg;
-                }
-            }
-            std::lock_guard<std::mutex> lk(mu);
-            if (!err.empty() && chunk_error[static_cast<size_t>(k)].empty()) chunk_error[static_cast<size_t>(k)] = err;
-            ++decoded[static_cast<size_t>(k)];
-            cv.notify_all();
-        }
-    };
-    std::vector<std::thread> pool;
-    try {
-        for (int t = 0; t < workers; ++t) pool.emplace_back(worker, t);
-    } catch (const std::exception& e) {
-        { std::lock_guard<std::mutex> lk(mu); abort = true; }
-        cv.notify_all();
-        for (auto& th : pool) th.join();
-        mdc_set_error("mdc_seq_prepare_device: cannot start decode threads (%s)", e.what());
-        return MDC_ERR_IO;
-    }
-
-    HostBatch batch[2];
-    DevSlot dev[2];
-    cudaEvent_t ev_status[2] = {nullptr, nullptr}, ev_done[2] = {nullptr, nullptr};
-    uint32_t* status_pinned[2] = {nullptr, nullptr};
+    std::vector<int> ids(static_cast<size_t>(count));
+    for (int i = 0; i < count; ++i) ids[static_cast<size_t>(i)] = first + i;
     std::string fail_msg;
-    int rc = MDC_OK;
-    for (int b = 0; b < 2 && rc == MDC_OK; ++b)
-        if (cudaEventCreateWithFlags(&ev_status[b], cudaEventDisableTiming) != cudaSuccess ||
-            cudaEventCreateWithFlags(&ev_done[b], cudaEventDisableTiming) != cudaSuccess ||
-            cudaEventRecord(ev_done[b], st) != cudaSuccess) {
-            mdc_set_error("mdc_seq_prepare_device: cannot create events");
-            rc = MDC_ERR_CUDA;
-        }
-    // chunk k: pack into pinned staging, then H2D -> J1 -> J2 (-> status D2H) on the stream
-    auto submit = [&](int k) -> int {
-        const int b = k & 1, f0 = k * chunk, n = std::min(chunk, count - f0);
-        HostBatch& hb = batch[b];
-        hb = HostBatch();
-        std::vector<size_t> at(static_cast<size_t>(n));
-        for (int i = 0; i < n; ++i) {
-            FeedFrame& ff = frames[b][static_cast<size_t>(i)];
-            at[static_cast<size_t>(i)] = hb.bytes;
-            if (ff.jpeg) {
-                hb.add_jpeg(*ff.hdr, ff.segs, ff.complete, mdc_seq_name(s, first + f0 + i), hb.bytes);
-                hb.bytes += ff.segs.empty() ? 0 : ff.segs.back().end - ff.segs.front().begin;
-            } else {
-                hb.add_raw(hb.bytes);
-                hb.bytes += ff.px.size();
-            }
-        }
-        const size_t meta = hb.meta_bytes(), need = meta + HostBatch::align(hb.bytes) + sizeof(uint32_t) * static_cast<size_t>(n);
-        // the slot's previous chunk (k - 2) has left the staging buffer and the device buffers behind
-        CU_CHECK(cudaEventSynchronize(ev_done[b]));
-        if (stage->bytes[b] < need) {
-            if (stage->pinned[b]) mdc_host_free(stage->pinned[b]);
-            stage->pinned[b] = nullptr;
-            stage->bytes[b] = 0;
-            if (mdc_host_alloc(&stage->pinned[b], need + need / 8) != MDC_OK) return MDC_ERR_CUDA;
-            stage->bytes[b] = need + need / 8;
-        }
-        int r = prepare_slot(hb, dev[b]);
-        if (r == MDC_OK) r = grow(&dev[b].u8, &dev[b].u8_cap, static_cast<size_t>(chunk) * in_h * pitch);
-        if (r != MDC_OK) return r;
-        uint8_t* pin = static_cast<uint8_t*>(stage->pinned[b]);
-        hb.write_meta(pin, dev[b].meta);
-        for (int i = 0; i < n; ++i) {
-            const FeedFrame& ff = frames[b][static_cast<size_t>(i)];
-            uint8_t* dst = pin + meta + at[static_cast<size_t>(i)];
-            if (ff.jpeg && !ff.segs.empty()) memcpy(dst, ff.file.data() + ff.segs.front().begin, ff.segs.back().end - ff.segs.front().begin);
-            else if (!ff.jpeg) memcpy(dst, ff.px.data(), ff.px.size());
-        }
-        status_pinned[b] = reinterpret_cast<uint32_t*>(pin + meta + HostBatch::align(hb.bytes));
-        r = enqueue_batch(hb, dev[b], pin, pin + meta, in_w, in_h, dev[b].u8, pitch, status_pinned[b], st);
-        if (r != MDC_OK) return r;
-        CU_CHECK(cudaEventRecord(ev_status[b], st));
-        return MDC_OK;
-    };
-    // chunk k after J1 / J2: a frame that failed stops the call before its chunk reaches K1; otherwise K1 into the level buffers
-    auto finish = [&](int k) -> int {
-        const int b = k & 1, f0 = k * chunk, n = std::min(chunk, count - f0);
-        CU_CHECK(cudaEventSynchronize(ev_status[b]));
-        for (int i = 0; i < n; ++i) {
-            std::string m;
-            if (status_pinned[b][i] != kStatusOk) m = std::string(mdc_seq_name(s, first + f0 + i)) + ": " + kind_message(status_pinned[b][i]);
-            else m = batch[b].incomplete_msg[static_cast<size_t>(i)];
-            if (!m.empty()) { fail_msg = m; return MDC_ERR_FORMAT; }
-        }
+    // a frame that failed stops the call before its chunk reaches K1; otherwise K1 into the level buffers
+    auto prepare = [&](const FeedChunk& fc) -> int {
+        for (int i = 0; i < fc.n; ++i)
+            if (fc.status[static_cast<size_t>(i)] != MDC_OK) { fail_msg = fc.msg[static_cast<size_t>(i)]; return MDC_ERR_FORMAT; }
         std::vector<float*> outs(static_cast<size_t>(levels));
-        for (int l = 0; l < levels; ++l) outs[static_cast<size_t>(l)] = d_out_levels[l] ? d_out_levels[l] + static_cast<size_t>(f0) * level_px[static_cast<size_t>(l)] : nullptr;
-        const int r = mdc_prepare_batch_pitched(c, dev[b].u8, pitch, n, flags, outs.data(), levels, st);
-        if (r != MDC_OK) return r;
-        CU_CHECK(cudaEventRecord(ev_done[b], st));
-        return MDC_OK;
+        for (int l = 0; l < levels; ++l) outs[static_cast<size_t>(l)] = d_out_levels[l] ? d_out_levels[l] + static_cast<size_t>(fc.f0) * level_px[static_cast<size_t>(l)] : nullptr;
+        return mdc_prepare_batch_pitched(c, fc.frames, pitch, fc.n, flags, outs.data(), levels, st);
     };
-    for (int k = 0; k < n_chunks && rc == MDC_OK; ++k) {
-        std::string host_err;
-        {
-            std::unique_lock<std::mutex> lk(mu);
-            cv.wait(lk, [&] { return decoded[static_cast<size_t>(k)] == workers; });
-            host_err = chunk_error[static_cast<size_t>(k)];
-        }
-        if (host_err.empty()) {
-            rc = submit(k);
-            std::lock_guard<std::mutex> lk(mu);
-            released = k + 2;             // frames[k & 1] is packed: chunk k + 2 may be read into it
-            cv.notify_all();
-        }
-        if (rc == MDC_OK && k > 0) rc = finish(k - 1);          // overlaps chunk k's J1 / J2 on the GPU
-        if (rc == MDC_OK && !host_err.empty()) { fail_msg = host_err; rc = MDC_ERR_FORMAT; }
-        if (rc == MDC_OK && k == n_chunks - 1) rc = finish(k);
-    }
-    {
-        std::lock_guard<std::mutex> lk(mu);
-        abort = true;
-    }
-    cv.notify_all();
-    for (auto& th : pool) th.join();
-    const cudaError_t drained = cudaStreamSynchronize(st);
-    if (rc == MDC_OK && drained != cudaSuccess) { mdc_set_error("mdc_seq_prepare_device: %s", cudaGetErrorString(drained)); rc = MDC_ERR_CUDA; }
+    const int rc = run_device_feed(s, ids.data(), count, in_w, in_h, threads, nullptr, pitch, st, prepare, "mdc_seq_prepare_device");
     if (rc == MDC_ERR_FORMAT) {
         printf("ERROR: %s\n", fail_msg.c_str());
         mdc_set_error("mdc_seq_prepare_device: %s", fail_msg.c_str());
     }
-    for (int b = 0; b < 2; ++b) {
-        dev[b].release();
-        if (ev_status[b]) cudaEventDestroy(ev_status[b]);
-        if (ev_done[b]) cudaEventDestroy(ev_done[b]);
-    }
     return rc;
+}
+
+extern "C" int mdc_seq_read_gray8_device(mdc_ctx* c, const mdc_seq* s, const int* ids, int n, int w, int h, uint8_t* d_out, size_t row_pitch,
+                                         int* status_host, int* sizes_host, int threads, mdc_stream stream) {
+    if (n < 0 || (n > 0 && (!c || !s || !ids || !d_out)) || w < 1 || h < 1 || row_pitch < static_cast<size_t>(w)) {
+        mdc_set_error("mdc_seq_read_gray8_device: bad argument");
+        return MDC_ERR_INVALID_ARG;
+    }
+    const int n_files = mdc_seq_num_images(s);
+    for (int k = 0; k < n; ++k)
+        if (ids[k] < 0 || ids[k] >= n_files) {
+            mdc_set_error("mdc_seq_read_gray8_device: frame id %d (ids[%d]) outside the sequence's %d", ids[k], k, n_files);
+            return MDC_ERR_INVALID_ARG;
+        }
+    if (n == 0) return MDC_OK;
+    if (threads < 1) threads = mdc_seq_default_threads();
+    CU_CHECK(cudaSetDevice(mdc_ctx_device_ordinal(c)));
+    cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : static_cast<cudaStream_t>(mdc_ctx_stream_handle(c));
+    int first_bad = -1;
+    std::string first_msg;
+    // every frame's outcome is recorded; J2 has already written the rows of the frames that read
+    auto record = [&](const FeedChunk& fc) -> int {
+        for (int i = 0; i < fc.n; ++i) {
+            const int k = fc.f0 + i;
+            if (status_host) status_host[k] = fc.status[static_cast<size_t>(i)];
+            if (sizes_host) { sizes_host[2 * k] = fc.sizes[2 * static_cast<size_t>(i)]; sizes_host[2 * k + 1] = fc.sizes[2 * static_cast<size_t>(i) + 1]; }
+            if (fc.status[static_cast<size_t>(i)] != MDC_OK && first_bad < 0) { first_bad = k; first_msg = fc.msg[static_cast<size_t>(i)]; }
+        }
+        return MDC_OK;
+    };
+    const int rc = run_device_feed(s, ids, n, w, h, threads, d_out, row_pitch, st, record, "mdc_seq_read_gray8_device");
+    if (rc != MDC_OK) return rc;
+    if (first_bad >= 0) { mdc_set_error("%s", first_msg.c_str()); return MDC_ERR_FORMAT; }
+    return MDC_OK;
 }

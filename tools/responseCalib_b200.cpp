@@ -45,40 +45,46 @@ int main(int argc, char** argv) {
     for (int i = 2; i < argc; ++i) parse_option(argv[i], &opt);
     if (opt.skip < 1) opt.skip = 1;
 
-    // ---- the exposure sweep: every skip-th frame that decodes, with its exposure time
+    // ---- the exposure sweep: every skip-th frame that decodes, with its exposure time.  The first one that decodes sets the size
+    // (main_responseCalib.cpp:192-205); all of them are decoded in one call (JPEG frames on the GPU) into the device stack, and
+    // frames that cannot be decoded are skipped.
     mdc_seq* seq = nullptr;
     if (mdc_seq_open(argv[1], &seq) != MDC_OK) { printf("cannot open dataset %s: %s\n", argv[1], mdc_last_error()); return 1; }
+    std::vector<int> ids;
+    for (int i = 0; i < mdc_seq_num_images(seq); i += opt.skip) ids.push_back(i);
     int w = 0, h = 0;
-    std::vector<unsigned char> stack;
+    for (int i : ids)
+        if (mdc_seq_read_gray8(seq, i, nullptr, 0, &w, &h) == MDC_OK) break;       // leaves w, h at 0 if it fails
     std::vector<double> exposures;
-    std::vector<unsigned char> frame;
-    for (int i = 0; i < mdc_seq_num_images(seq); i += opt.skip) {
-        int fw = 0, fh = 0;
-        if (mdc_seq_read_gray8(seq, i, nullptr, 0, &fw, &fh) != MDC_OK || fw < 1 || fh < 1) continue;      // undecodable frame: skipped
-        if (w != 0 && fw != w) { printf("width mismatch!\n"); return 1; }
-        if (h != 0 && fh != h) { printf("height mismatch!\n"); return 1; }
-        w = fw; h = fh;
-        frame.resize(static_cast<size_t>(w) * h);
-        if (mdc_seq_read_gray8(seq, i, frame.data(), frame.size(), &fw, &fh) != MDC_OK) continue;
-        stack.insert(stack.end(), frame.begin(), frame.end());
-        exposures.push_back(static_cast<double>(mdc_seq_exposure(seq, i)));
+    mdc_ctx* ctx = nullptr;
+    unsigned char* d_data = nullptr;
+    if (w > 0) {
+        CUDA_OR_DIE(cudaSetDevice(opt.device));
+        MDC_OR_DIE(mdc_ctx_create(opt.device, nullptr, nullptr, &ctx));
+        const size_t frame_bytes = static_cast<size_t>(w) * h;
+        CUDA_OR_DIE(cudaMalloc(&d_data, frame_bytes * ids.size()));
+        std::vector<int> status(ids.size()), sizes(2 * ids.size());
+        const int r = mdc_seq_read_gray8_device(ctx, seq, ids.data(), static_cast<int>(ids.size()), w, h, d_data, w, status.data(), sizes.data(), 0, nullptr);
+        if (r != MDC_OK && r != MDC_ERR_FORMAT) { printf("mdc_seq_read_gray8_device failed (%d): %s\n", r, mdc_last_error()); exit(2); }
+        for (size_t k = 0; k < ids.size(); ++k) {
+            if (status[k] == MDC_ERR_FORMAT) continue;                                                    // undecodable frame: skipped
+            if (sizes[2 * k] != w) { printf("width mismatch!\n"); return 1; }
+            if (sizes[2 * k + 1] != h) { printf("height mismatch!\n"); return 1; }
+            const size_t n = exposures.size();
+            if (n != k) CUDA_OR_DIE(cudaMemcpy(d_data + n * frame_bytes, d_data + k * frame_bytes, frame_bytes, cudaMemcpyDeviceToDevice));
+            exposures.push_back(static_cast<double>(mdc_seq_exposure(seq, ids[k])));
+        }
     }
     const int n = static_cast<int>(exposures.size());
     const int npix = w * h;
     printf("loaded %d images\n", n);
     if (n < 1) return 1;
 
-    // ---- device state: image stack, exposure times, irradiance E, inverse response G
-    CUDA_OR_DIE(cudaSetDevice(opt.device));
-    mdc_ctx* ctx = nullptr;
-    MDC_OR_DIE(mdc_ctx_create(opt.device, nullptr, nullptr, &ctx));
-    unsigned char* d_data = nullptr;
+    // ---- device state: image stack (above), exposure times, irradiance E, inverse response G
     double *d_t = nullptr, *d_E = nullptr, *d_G = nullptr;
-    CUDA_OR_DIE(cudaMalloc(&d_data, stack.size()));
     CUDA_OR_DIE(cudaMalloc(&d_t, sizeof(double) * n));
     CUDA_OR_DIE(cudaMalloc(&d_E, sizeof(double) * npix));
     CUDA_OR_DIE(cudaMalloc(&d_G, sizeof(double) * 256));
-    CUDA_OR_DIE(cudaMemcpy(d_data, stack.data(), stack.size(), cudaMemcpyHostToDevice));
     CUDA_OR_DIE(cudaMemcpy(d_t, exposures.data(), sizeof(double) * n, cudaMemcpyHostToDevice));
     MDC_OR_DIE(mdc_rc_leak_padding(ctx, d_data, n, w, h, opt.leak_padding, nullptr));
 

@@ -7,12 +7,15 @@
 // projection + distortion + visibility mask of the plane grid (mdc_vc_plane_maps), and the loop (mdc_vignette_calib).
 //
 // The homographies from the unit square to the marker (:231-262) come from one of two places:
-//   homographies=detect  the tool detects the marker itself: raw frame -> rectification (mdc_prepare_batch, MDC_RECTIFY) -> 8-bit
+//   homographies=detect  the tool detects the marker itself: every skip-th frame decoded once into device memory
+//                        (mdc_seq_read_gray8_device) -> rectification (mdc_prepare_batch_pitched, MDC_RECTIFY) -> 8-bit
 //                        frame and adaptive threshold (mdc_marker_threshold) on the GPU, in chunks of frames; then aruco's
 //                        detector (mdc_marker_detect) on host threads, one frame per thread, and mdc_marker_homography.  The rows
 //                        it used are written to vignetteCalibResult/homographies.txt, in the format homographies=FILE reads.
 //   homographies=FILE    nine whitespace-separated numbers (the row-major 3x3 homography from marker corners to rectified pixels)
 //                        per considered frame i = 0, skip, 2*skip, ...
+// The frames that have a homography are decoded in one mdc_seq_read_gray8_device call (JPEG frames on the GPU), or, after detection,
+// gathered from the frames it decoded.
 // A row containing NaN means that the frame does not show exactly one marker: the frame is left out (:240), but its exposure
 // still counts in the mean exposure, as in the reference.  The debug overlays and imshow windows (:306-368) are not produced.
 //
@@ -135,17 +138,35 @@ bool write_plane_png(const std::string& path, const std::vector<float>& I, int w
     return write_png(path, px, w, h, 8, 2);
 }
 
+// Every skip-th frame (ids) decoded into the device stack d_stack [ids][hI][pitch] in one call; exits at the first one that cannot be
+// read as a wI x hI image, with the reader's message.
+void read_frames(mdc_ctx* ctx, mdc_seq* seq, const std::vector<int>& ids, int wI, int hI, uint8_t* d_stack, size_t pitch) {
+    std::vector<int> status(ids.size());
+    const int r = mdc_seq_read_gray8_device(ctx, seq, ids.data(), static_cast<int>(ids.size()), wI, hI, d_stack, pitch, status.data(), nullptr, 0, nullptr);
+    if (r != MDC_OK && r != MDC_ERR_FORMAT) { printf("mdc_seq_read_gray8_device failed (%d): %s\n", r, mdc_last_error()); exit(2); }
+    for (size_t k = 0; k < ids.size(); ++k)
+        if (status[k] != MDC_OK) {
+            printf("frame %d: cannot read a %dx%d image: %s\n", ids[k], wI, hI, mdc_last_error());       // the first failed frame's message
+            exit(1);
+        }
+}
+
 // Homographies of frames i = 0, skip, ... by marker detection; writes them (NaN rows for frames without exactly one marker) to `out`.
-void detect_homographies(mdc_ctx* ctx, mdc_seq* seq, int skip, int wI, int hI, int w_out, int h_out, const char* out) {
+// The frames are decoded once into *d_stack ([ids][hI][pitch], rows padded to 16 bytes so that the rectification keeps its TMA loader),
+// which the caller gathers the frames with a marker from.
+void detect_homographies(mdc_ctx* ctx, mdc_seq* seq, int skip, int wI, int hI, int w_out, int h_out, const char* out, uint8_t** d_stack, size_t* pitch) {
     const int num_images = mdc_seq_num_images(seq);
     std::vector<int> ids;
     for (int i = 0; i < num_images; i += skip) ids.push_back(i);
+    *pitch = (static_cast<size_t>(wI) + 15) / 16 * 16;
+    const size_t frame_bytes = *pitch * hI;
+    CUDA_OR_DIE(cudaMalloc(d_stack, std::max<size_t>(1, frame_bytes * ids.size())));
+    read_frames(ctx, seq, ids, wI, hI, *d_stack, *pitch);
     const size_t npx_in = static_cast<size_t>(wI) * hI, npx = static_cast<size_t>(w_out) * h_out;
     const int chunk = static_cast<int>(std::max<size_t>(1, std::min<size_t>(32, (size_t(1) << 30) / (npx * 4 + npx_in))));
-    std::vector<uint8_t> raw(chunk * npx_in), grey(chunk * npx), mask(chunk * npx);
-    uint8_t *d_raw = nullptr, *d_grey = nullptr, *d_mask = nullptr;
+    std::vector<uint8_t> grey(chunk * npx), mask(chunk * npx);
+    uint8_t *d_grey = nullptr, *d_mask = nullptr;
     float* d_rect = nullptr;
-    CUDA_OR_DIE(cudaMalloc(&d_raw, raw.size()));
     CUDA_OR_DIE(cudaMalloc(&d_rect, chunk * npx * sizeof(float)));
     CUDA_OR_DIE(cudaMalloc(&d_grey, grey.size()));
     CUDA_OR_DIE(cudaMalloc(&d_mask, mask.size()));
@@ -154,15 +175,7 @@ void detect_homographies(mdc_ctx* ctx, mdc_seq* seq, int skip, int wI, int hI, i
     int found = 0;
     for (size_t first = 0; first < ids.size(); first += chunk) {
         const int m = static_cast<int>(std::min<size_t>(chunk, ids.size() - first));
-        for (int k = 0; k < m; ++k) {
-            int fw = 0, fh = 0;
-            if (mdc_seq_read_gray8(seq, ids[first + k], raw.data() + k * npx_in, npx_in, &fw, &fh) != MDC_OK || fw != wI || fh != hI) {
-                printf("frame %d: cannot read a %dx%d image: %s\n", ids[first + k], wI, hI, mdc_last_error());
-                exit(1);
-            }
-        }
-        CUDA_OR_DIE(cudaMemcpy(d_raw, raw.data(), m * npx_in, cudaMemcpyHostToDevice));
-        MDC_OR_DIE(mdc_prepare_batch(ctx, d_raw, m, MDC_RECTIFY, &d_rect, 1, nullptr));           // getImage(i, true, false, false, false)
+        MDC_OR_DIE(mdc_prepare_batch_pitched(ctx, *d_stack + first * frame_bytes, *pitch, m, MDC_RECTIFY, &d_rect, 1, nullptr));   // getImage(i, true, false, false, false)
         MDC_OR_DIE(mdc_marker_threshold(ctx, d_rect, m, w_out, h_out, d_grey, d_mask, nullptr));
         CUDA_OR_DIE(cudaMemcpy(grey.data(), d_grey, m * npx, cudaMemcpyDeviceToHost));
         CUDA_OR_DIE(cudaMemcpy(mask.data(), d_mask, m * npx, cudaMemcpyDeviceToHost));
@@ -187,7 +200,7 @@ void detect_homographies(mdc_ctx* ctx, mdc_seq* seq, int skip, int wI, int hI, i
             found += !std::isnan(Hs[(first + k) * 9]);
         }
     }
-    cudaFree(d_raw); cudaFree(d_rect); cudaFree(d_grey); cudaFree(d_mask);
+    cudaFree(d_rect); cudaFree(d_grey); cudaFree(d_mask);
     printf("found exactly one marker in %d of %zu frames\n", found, ids.size());
     FILE* f = fopen(out, "w");
     if (!f) { printf("cannot write %s\n", out); exit(1); }
@@ -235,41 +248,52 @@ int main(int argc, char** argv) {
     CUDA_OR_DIE(cudaSetDevice(opt.device));
     mdc_ctx* ctx = nullptr;
     MDC_OR_DIE(mdc_ctx_create(opt.device, fov, photo, &ctx));
+    uint8_t* d_stack = nullptr;            // homographies=detect: every skip-th frame, decoded for the detection
+    size_t stack_pitch = 0;
     if (opt.homographies == "detect") {
         opt.homographies = "vignetteCalibResult/homographies.txt";
-        detect_homographies(ctx, seq, opt.skip, wI, hI, w_out, h_out, opt.homographies.c_str());
+        detect_homographies(ctx, seq, opt.skip, wI, hI, w_out, h_out, opt.homographies.c_str(), &d_stack, &stack_pitch);
     }
 
-    // ---- frames that have a homography
+    // ---- frames that have a homography, as [n][wI*hI] on the device: gathered from the detection's stack, or decoded in one call
     FILE* hf = fopen(opt.homographies.c_str(), "r");
     if (!hf) { printf("cannot open %s\n", opt.homographies.c_str()); return 1; }
     const size_t npx = static_cast<size_t>(wI) * hI;
-    std::vector<uint8_t> stack, frame(npx);
+    std::vector<int> ids;
     std::vector<float> exposures;
     std::vector<double> Hs;
+    int missing = -1;                      // first frame without a row: reported after the frames before it have been read
     for (int i = 0; i < num_images; i += opt.skip) {
         double H[9];
-        for (int k = 0; k < 9; ++k)
-            if (fscanf(hf, "%lf", &H[k]) != 1) { printf("%s: no homography for frame %d\n", opt.homographies.c_str(), i); return 1; }
+        bool complete = true;
+        for (int k = 0; k < 9 && complete; ++k) complete = fscanf(hf, "%lf", &H[k]) == 1;
+        if (!complete) { missing = i; break; }
         bool found = true;
         for (double v : H) found = found && !std::isnan(v);
         if (!found) continue;                                   // no marker in this frame (:240)
-        int fw = 0, fh = 0;
-        if (mdc_seq_read_gray8(seq, i, frame.data(), frame.size(), &fw, &fh) != MDC_OK || fw != wI || fh != hI) {
-            printf("frame %d: cannot read a %dx%d image: %s\n", i, wI, hI, mdc_last_error());
-            return 1;
-        }
-        stack.insert(stack.end(), frame.begin(), frame.end());
+        ids.push_back(i);
         exposures.push_back(mdc_seq_exposure(seq, i));
         Hs.insert(Hs.end(), H, H + 9);
     }
     fclose(hf);
+    uint8_t* d_frames = nullptr;
+    if (!ids.empty()) {
+        CUDA_OR_DIE(cudaMalloc(&d_frames, npx * ids.size()));
+        if (!d_stack) {
+            read_frames(ctx, seq, ids, wI, hI, d_frames, wI);
+        } else {
+            for (size_t k = 0; k < ids.size(); ++k)
+                CUDA_OR_DIE(cudaMemcpy2D(d_frames + k * npx, wI, d_stack + static_cast<size_t>(ids[k] / opt.skip) * stack_pitch * hI, stack_pitch, wI, hI,
+                                         cudaMemcpyDeviceToDevice));
+        }
+    }
+    cudaFree(d_stack);
+    if (missing >= 0) { printf("%s: no homography for frame %d\n", opt.homographies.c_str(), missing); return 1; }
     const int n = static_cast<int>(exposures.size());
     printf("loaded %d images with a marker\n", n);
     const size_t gwgh = static_cast<size_t>(opt.gw) * opt.gh;
 
     // ---- front end on the device: gamma removal, normalisation + gradient invalidation, plane-to-image maps
-    uint8_t* d_frames = nullptr;
     float *d_images = nullptr, *d_p2x = nullptr, *d_p2y = nullptr, *d_plane = nullptr, *d_vig = nullptr, *d_smoothed = nullptr;
     CUDA_OR_DIE(cudaMalloc(&d_images, npx * n * sizeof(float) + 4));
     CUDA_OR_DIE(cudaMalloc(&d_p2x, gwgh * n * sizeof(float) + 4));
@@ -278,8 +302,6 @@ int main(int argc, char** argv) {
     CUDA_OR_DIE(cudaMalloc(&d_vig, npx * sizeof(float)));
     CUDA_OR_DIE(cudaMalloc(&d_smoothed, npx * sizeof(float)));
     if (n > 0) {
-        CUDA_OR_DIE(cudaMalloc(&d_frames, stack.size()));
-        CUDA_OR_DIE(cudaMemcpy(d_frames, stack.data(), stack.size(), cudaMemcpyHostToDevice));
         MDC_OR_DIE(mdc_unmap_u8(ctx, d_frames, d_images, static_cast<int>(npx), n, MDC_REMOVE_GAMMA, nullptr));      // getImage(i,false,true,false,false)
         CUDA_OR_DIE(cudaFree(d_frames));
         MDC_OR_DIE(mdc_vc_prepare_images(ctx, d_images, n, wI, hI, exposures.data(), mean_exposure, 255, d_images, nullptr));
