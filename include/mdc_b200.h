@@ -46,6 +46,17 @@ extern "C" {
 
 #define MDC_MAX_PYR_LEVELS 8
 
+/* Element type of prepared levels (the out_type of the mdc_*_ex calls).  Every level is computed in fp32 exactly as for
+ * MDC_OUT_F32 and converted when it is stored; no level is ever computed from a converted one:
+ *   MDC_OUT_F32  float, the getImage result itself
+ *   MDC_OUT_F16  IEEE binary16, round to nearest even (__float2half_rn; numpy astype(float16), torch .to(float16)): NaN stays NaN,
+ *                a value above 65504 after rounding becomes +-inf
+ *   MDC_OUT_U8   uint8 as cv::Mat::convertTo(CV_8U) (saturate_cast<uchar>(float)) does it on x86-64: round half to even, NaN,
+ *                +-inf and values outside int32 become 0, anything else is clamped to [0, 255] */
+#define MDC_OUT_F32 0
+#define MDC_OUT_F16 1
+#define MDC_OUT_U8 2
+
 typedef struct mdc_fov mdc_fov;     /* host-side FOV rectifier model  (UndistorterFOV state)          */
 typedef struct mdc_photo mdc_photo; /* host-side photometric model    (PhotometricUndistorter state)  */
 typedef struct mdc_ctx mdc_ctx;     /* device context: tables resident in HBM + tile plan + streams   */
@@ -196,6 +207,17 @@ int mdc_prepare_batch(mdc_ctx* c, const uint8_t* d_frames, int n_frames, unsigne
 int mdc_prepare_batch_pitched(mdc_ctx* c, const uint8_t* d_frames, size_t row_pitch_bytes, int n_frames, unsigned flags,
                               float* const* d_out_levels, int levels, mdc_stream stream);
 
+/* The same getImage + pyramid with the levels stored as out_type (MDC_OUT_F32 / MDC_OUT_F16 / MDC_OUT_U8): level l of type T is
+ * conv_T of what the same call with MDC_OUT_F32 gives, pixel for pixel (see MDC_OUT_*); the conversion happens in the kernels' stores,
+ * so the call launches exactly the kernels the fp32 call launches.  d_out_levels[l]: [n_frames][w_l*h_l] elements of out_type.
+ * row_pitch_bytes = 0: tightly packed input rows (mdc_prepare_batch), else as mdc_prepare_batch_pitched.  Narrow types keep the levels
+ * a K2 pass reads (level 2 when levels > 3; every level but the last in non-rectifying mode) in fp32 scratch that the call takes from a
+ * memory pool of the context, stream-ordered on `stream`.  An unknown out_type returns MDC_ERR_INVALID_ARG before anything else is
+ * looked at; every other argument rule is that of mdc_prepare_batch(_pitched).  mdc_prepare_batch(_pitched) is this call with
+ * MDC_OUT_F32. */
+int mdc_prepare_batch_ex(mdc_ctx* c, const uint8_t* d_frames, size_t row_pitch_bytes, int n_frames, unsigned flags, int out_type,
+                         void* const* d_out_levels, int levels, mdc_stream stream);
+
 /* Stand-alone pyramid level (kernel K2): dst[x,y] = 0.25f*(((a+b)+c)+d) over the 2x2 block. */
 int mdc_pyr_down(mdc_ctx* c, const float* d_src, int src_w, int src_h, float* d_dst, int n_frames, mdc_stream stream);
 
@@ -226,6 +248,10 @@ int mdc_seq_read_gray8(const mdc_seq* s, int id, uint8_t* out, size_t capacity, 
  * rows from that chunk on are not written.  first / count outside the sequence, levels outside 1..MDC_MAX_PYR_LEVELS or a NULL
  * level that has pixels (a level without pixels may be NULL) return MDC_ERR_INVALID_ARG before anything is decoded. */
 int mdc_seq_prepare(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned flags, float* const* h_out_levels, int levels, int threads);
+/* mdc_seq_prepare with the levels stored as out_type (MDC_OUT_*, as for mdc_prepare_batch_ex); h_out_levels[l] holds count*w_l*h_l
+ * elements of that type.  An unknown out_type returns MDC_ERR_INVALID_ARG before any other check; everything else as mdc_seq_prepare. */
+int mdc_seq_prepare_ex(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned flags, int out_type, void* const* h_out_levels,
+                       int levels, int threads);
 /* The same getImage for [first, first+count) into DEVICE level buffers (level l: [count][(w>>l)*(h>>l)] floats), with the JPEG frames
  * decoded on the GPU: `threads` host threads (0 = all) read the files, parse the JPEG headers and split the scans into restart intervals,
  * and the main thread packs the entropy-coded bytes of a chunk into pinned staging; each chunk then goes H2D -> entropy decode (J1) ->
@@ -236,6 +262,9 @@ int mdc_seq_prepare(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned
  * are complete, and nothing from its chunk on is written.  Returns when the work is done on the device. */
 int mdc_seq_prepare_device(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned flags, float* const* d_out_levels, int levels,
                            int threads, mdc_stream stream);
+/* mdc_seq_prepare_device with the levels stored as out_type (as mdc_seq_prepare_ex); the same bytes as mdc_seq_prepare_ex. */
+int mdc_seq_prepare_device_ex(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned flags, int out_type, void* const* d_out_levels,
+                              int levels, int threads, mdc_stream stream);
 /* getImageRaw_internal(ids[k]) for k < n into DEVICE memory: frame k -> d_out + k*h*row_pitch (row_pitch >= w; a multiple of 16 keeps
  * mdc_prepare_batch_pitched on its TMA loader).  ids may be in any order and may repeat.  The same device feed as mdc_seq_prepare_device
  * (`threads` host threads, 0 = the default count; chunks of min(512, max(16, 32 * threads)) frames; JPEG frames decoded on the GPU,
@@ -437,6 +466,11 @@ int mdc_undistort_f32_host(mdc_ctx* c, const float* in, float* out, int n_pix_in
  * after the last copy into out_levels has landed. */
 int mdc_prepare_batch_host(mdc_ctx* c, const uint8_t* frames, int n_frames, unsigned flags,
                            float* const* out_levels, int levels);
+/* The same with the levels stored as out_type (MDC_OUT_*, as for mdc_prepare_batch_ex): the device buffers of the pipeline and the
+ * copies back to out_levels move out_type elements, so F16 halves and U8 quarters the device-to-host bytes.  An unknown out_type
+ * returns MDC_ERR_INVALID_ARG before anything else. */
+int mdc_prepare_batch_host_ex(mdc_ctx* c, const uint8_t* frames, int n_frames, unsigned flags, int out_type, void* const* out_levels,
+                              int levels);
 /* Pinned host memory for the calling thread's current CUDA device, placed on the NUMA node that device is attached to
  * (MDC_NUMA_BIND=0 disables the placement). */
 int mdc_host_alloc(void** p, size_t bytes);

@@ -14,6 +14,7 @@ LIB_PATH = os.path.join(PKG, "lib", "libmdc_b200.so")
 MDC_OK = 0
 ERR_NAMES = {1: "INVALID_ARG", 2: "IO", 3: "FORMAT", 4: "INVALID_OBJECT", 5: "CUDA", 6: "UNSUPPORTED"}
 RECTIFY, REMOVE_GAMMA, REMOVE_VIGNETTE, NAN_OVEREXPOSED = 1, 2, 4, 8
+OUT_F32, OUT_F16, OUT_U8 = 0, 1, 2          # element type of prepared levels (MDC_OUT_*)
 FOV_CROP, FOV_FULL, FOV_EXPLICIT = -1, -2, 0
 MAX_PYR_LEVELS = 8
 
@@ -46,6 +47,8 @@ SIGNATURES = {
     "mdc_seq_read_gray8": (C.c_int, [_vp, C.c_int, _vp, C.c_size_t, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "mdc_seq_prepare": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint, C.POINTER(_vp), C.c_int, C.c_int]),
     "mdc_seq_prepare_device": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint, C.POINTER(_vp), C.c_int, C.c_int, _vp]),
+    "mdc_seq_prepare_ex": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint, C.c_int, C.POINTER(_vp), C.c_int, C.c_int]),
+    "mdc_seq_prepare_device_ex": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint, C.c_int, C.POINTER(_vp), C.c_int, C.c_int, _vp]),
     "mdc_seq_read_gray8_device": (C.c_int, [_vp, _vp, _vp, C.c_int, C.c_int, C.c_int, _vp, C.c_size_t, _vp, _vp, C.c_int, _vp]),
     "mdc_jpeg_decode_device": (C.c_int, [_vp, C.POINTER(_vp), C.POINTER(C.c_size_t), C.c_int, C.c_int, C.c_int, _vp, C.c_size_t,
                                          C.POINTER(C.c_int), _vp]),
@@ -91,6 +94,7 @@ SIGNATURES = {
     "mdc_undistort_f32": (C.c_int, [_vp, _vp, _vp, C.c_int, C.c_int, C.c_int, _vp]),
     "mdc_prepare_batch": (C.c_int, [_vp, _vp, C.c_int, C.c_uint, C.POINTER(_vp), C.c_int, _vp]),
     "mdc_prepare_batch_pitched": (C.c_int, [_vp, _vp, C.c_size_t, C.c_int, C.c_uint, C.POINTER(_vp), C.c_int, _vp]),
+    "mdc_prepare_batch_ex": (C.c_int, [_vp, _vp, C.c_size_t, C.c_int, C.c_uint, C.c_int, C.POINTER(_vp), C.c_int, _vp]),
     "mdc_pyr_down": (C.c_int, [_vp, _vp, C.c_int, C.c_int, _vp, C.c_int, _vp]),
     "mdc_estep": (C.c_int, [_vp, _vp, C.c_int, C.c_int, _vp, _vp, _vp, _vp]),
     "mdc_rc_leak_padding": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp]),
@@ -109,6 +113,7 @@ SIGNATURES = {
     "mdc_undistort_u8_host": (C.c_int, [_vp, _vp, _vp, C.c_int, C.c_int]),
     "mdc_undistort_f32_host": (C.c_int, [_vp, _vp, _vp, C.c_int, C.c_int]),
     "mdc_prepare_batch_host": (C.c_int, [_vp, _vp, C.c_int, C.c_uint, C.POINTER(_vp), C.c_int]),
+    "mdc_prepare_batch_host_ex": (C.c_int, [_vp, _vp, C.c_int, C.c_uint, C.c_int, C.POINTER(_vp), C.c_int]),
     "mdc_host_alloc": (C.c_int, [C.POINTER(_vp), C.c_size_t]),
     "mdc_host_free": (None, [_vp]),
     "mdc_device_numa_node": (C.c_int, [C.c_int]),

@@ -29,6 +29,34 @@ def _is_torch(x) -> bool:
     return type(x).__module__.startswith("torch")
 
 
+_OUT_TYPES = {"float32": _lib.OUT_F32, "float16": _lib.OUT_F16, "uint8": _lib.OUT_U8}
+
+
+def _dtype_name(dtype) -> str:
+    """'float32' / 'float16' / 'uint8' / ... for a torch or numpy dtype (None = float32)."""
+    if dtype is None:
+        return "float32"
+    if type(dtype).__module__.startswith("torch"):
+        return str(dtype).split(".")[-1]
+    return np.dtype(dtype).name
+
+
+def _out_type(dtype) -> int:
+    """The MDC_OUT_* of a torch / numpy dtype; prepared levels come as float32 (default), float16 or uint8."""
+    name = _dtype_name(dtype)
+    if name not in _OUT_TYPES:
+        raise ValueError(f"prepared levels are float32, float16 or uint8, not {dtype}")
+    return _OUT_TYPES[name]
+
+
+def _check_out_dtype(outs, dtype):
+    """Caller-supplied level buffers must have the requested element type (raw integer addresses are taken as they are)."""
+    want = _dtype_name(dtype)
+    for i, o in enumerate(outs):
+        if hasattr(o, "dtype") and _dtype_name(o.dtype) != want:
+            raise ValueError(f"output level {i} is {o.dtype}, expected {want}")
+
+
 def _flags(rectify, gamma, vignette, nan_over) -> int:
     return (RECTIFY if rectify else 0) | (REMOVE_GAMMA if gamma else 0) | (REMOVE_VIGNETTE if vignette else 0) | \
         (NAN_OVEREXPOSED if nan_over else 0)
@@ -308,19 +336,25 @@ class Context:
         torch.cuda.current_stream(t.device).synchronize()
 
     # ---- device-resident operators (CUDA tensors, asynchronous on torch's current stream)
-    def prepare_batch(self, frames, flags: int, out_levels):
-        """frames: uint8 CUDA tensor [n, H*W] (or [n,H,W]); out_levels: list of float32 CUDA tensors."""
-        n = frames.shape[0]
-        arr = (C.c_void_p * len(out_levels))(*[t.data_ptr() for t in out_levels])
-        check(lib.mdc_prepare_batch(self._h, C.c_void_p(frames.data_ptr()), n, flags, arr, len(out_levels), self._stream(frames)),
-              "mdc_prepare_batch")
+    def prepare_batch(self, frames, flags: int, out_levels, dtype=None):
+        """frames: uint8 CUDA tensor [n, H*W] (or [n,H,W]); out_levels: list of CUDA tensors of `dtype` (torch.float32 (default),
+        torch.float16 or torch.uint8: the fp32 levels converted as MDC_OUT_F16 / MDC_OUT_U8 describe, inside the same kernels)."""
+        self._prepare(frames, 0, flags, out_levels, dtype)
 
-    def prepare_batch_pitched(self, frames, pitch: int, flags: int, out_levels):
-        """frames: uint8 CUDA tensor [n, H, pitch] whose rows hold in_w pixels followed by padding (rectifying mode only)."""
+    def prepare_batch_pitched(self, frames, pitch: int, flags: int, out_levels, dtype=None):
+        """frames: uint8 CUDA tensor [n, H, pitch] whose rows hold in_w pixels followed by padding (rectifying mode only).
+        out_levels and dtype as for prepare_batch."""
+        if pitch == 0:
+            raise ValueError("prepare_batch_pitched: row pitch 0 (use prepare_batch for tightly packed rows)")
+        self._prepare(frames, pitch, flags, out_levels, dtype)
+
+    def _prepare(self, frames, pitch, flags, out_levels, dtype):
+        out_type = _out_type(dtype)
+        _check_out_dtype(out_levels, dtype)
         n = frames.shape[0]
         arr = (C.c_void_p * len(out_levels))(*[t.data_ptr() for t in out_levels])
-        check(lib.mdc_prepare_batch_pitched(self._h, C.c_void_p(frames.data_ptr()), pitch, n, flags, arr, len(out_levels), self._stream(frames)),
-              "mdc_prepare_batch_pitched")
+        check(lib.mdc_prepare_batch_ex(self._h, C.c_void_p(frames.data_ptr()), pitch, n, flags, out_type, arr, len(out_levels),
+                                       self._stream(frames)), "mdc_prepare_batch")
 
     def unmap_device(self, image_in, image_out, n, flags, n_frames=1):
         check(lib.mdc_unmap_u8(self._h, C.c_void_p(image_in.data_ptr()), C.c_void_p(image_out.data_ptr()), n, n_frames, flags,
@@ -491,13 +525,17 @@ class Context:
         fn = lib.mdc_undistort_u8_host if inp.dtype == np.uint8 else lib.mdc_undistort_f32_host
         check(fn(self._h, inp.ctypes.data_as(C.c_void_p), out.ctypes.data_as(C.c_void_p), n_in, n_out), "mdc_undistort_host")
 
-    def prepare_batch_host(self, frames, flags: int, out_levels):
-        """frames / out_levels: numpy arrays or raw integer addresses of (pinned) host memory."""
+    def prepare_batch_host(self, frames, flags: int, out_levels, dtype=None):
+        """frames / out_levels: numpy arrays or raw integer addresses of (pinned) host memory; the levels hold `dtype` elements
+        (np.float32 (default), np.float16 or np.uint8, or the torch dtypes of those)."""
         def addr(x):
             return x if isinstance(x, int) else x.ctypes.data
+        out_type = _out_type(dtype)
+        _check_out_dtype(out_levels, dtype)
         n = frames.shape[0]
         arr = (C.c_void_p * len(out_levels))(*[addr(t) for t in out_levels])
-        check(lib.mdc_prepare_batch_host(self._h, C.c_void_p(addr(frames)), n, flags, arr, len(out_levels)), "mdc_prepare_batch_host")
+        check(lib.mdc_prepare_batch_host_ex(self._h, C.c_void_p(addr(frames)), n, flags, out_type, arr, len(out_levels)),
+              "mdc_prepare_batch_host")
 
 
 class ExposureImage:
@@ -559,26 +597,32 @@ class Sequence:
         return out
 
     def prepare(self, ctx: "Context", level_shapes, first: int, count: int, rectify, removeGamma, removeVignette, nanOverexposed,
-                threads: int = 0):
-        """getImage for frames [first, first+count) -> list of float32 arrays [count, w_l*h_l] (one per pyramid level)."""
-        outs = [np.empty((count, w * h), np.float32) for (w, h) in level_shapes]
+                threads: int = 0, dtype=None):
+        """getImage for frames [first, first+count) -> list of arrays [count, w_l*h_l] (one per pyramid level) of `dtype`
+        (np.float32 (default), np.float16 or np.uint8)."""
+        out_type = _out_type(dtype)
+        outs = [np.empty((count, w * h), _dtype_name(dtype)) for (w, h) in level_shapes]
         ptrs = (C.c_void_p * len(outs))(*[o.ctypes.data for o in outs])
-        check(lib.mdc_seq_prepare(ctx._h, self._h, first, count, _flags(rectify, removeGamma, removeVignette, nanOverexposed), ptrs, len(outs), threads),
-              "mdc_seq_prepare")
+        check(lib.mdc_seq_prepare_ex(ctx._h, self._h, first, count, _flags(rectify, removeGamma, removeVignette, nanOverexposed), out_type, ptrs,
+                                     len(outs), threads), "mdc_seq_prepare")
         return outs
 
     def prepare_device(self, ctx: "Context", first: int, count: int, rectify, removeGamma, removeVignette, nanOverexposed, levels: int = 1,
-                       threads: int = 0, out=None):
-        """getImage for frames [first, first+count) with the JPEG frames decoded on the GPU (mdc_seq_prepare_device) -> list of float32
-        CUDA tensors [count, w_l*h_l] on the context's device, one per pyramid level.  Runs on torch's current stream."""
+                       threads: int = 0, out=None, dtype=None):
+        """getImage for frames [first, first+count) with the JPEG frames decoded on the GPU (mdc_seq_prepare_device) -> list of CUDA
+        tensors [count, w_l*h_l] of `dtype` (torch.float32 (default), torch.float16 or torch.uint8) on the context's device, one per
+        pyramid level.  Runs on torch's current stream."""
         import torch
+        out_type = _out_type(dtype)
         if out is None:
             w, h = ctx.level_dims(0) if rectify else ctx.in_dims
-            out = [torch.empty((count, (w >> l) * (h >> l)), dtype=torch.float32, device=f"cuda:{ctx.device}") for l in range(levels)]
+            tdt = getattr(torch, _dtype_name(dtype))
+            out = [torch.empty((count, (w >> l) * (h >> l)), dtype=tdt, device=f"cuda:{ctx.device}") for l in range(levels)]
+        _check_out_dtype(out, dtype)
         ptrs = (C.c_void_p * len(out))(*[t.data_ptr() for t in out])
         stream = Context._stream(out[0]) if out else None
-        check(lib.mdc_seq_prepare_device(ctx._h, self._h, first, count, _flags(rectify, removeGamma, removeVignette, nanOverexposed), ptrs,
-                                         len(out), threads, stream), "mdc_seq_prepare_device")
+        check(lib.mdc_seq_prepare_device_ex(ctx._h, self._h, first, count, _flags(rectify, removeGamma, removeVignette, nanOverexposed), out_type,
+                                            ptrs, len(out), threads, stream), "mdc_seq_prepare_device")
         return out
 
     def read_gray8_device(self, ctx: "Context", ids, w: int, h: int, row_pitch: int | None = None, threads: int = 0, out=None):
@@ -642,13 +686,16 @@ class FramePreparer:
         w, h = (self.width, self.height) if rectify else (self.widthOrg, self.heightOrg)
         return [(w >> l, h >> l) for l in range(levels)]
 
-    def prepare_device(self, frames, rectify, removeGamma, removeVignette, nanOverexposed, levels: int = 1, out=None):
-        """Batched, device-resident getImage (+ pyramid): frames uint8 CUDA tensor [n, H*W]."""
+    def prepare_device(self, frames, rectify, removeGamma, removeVignette, nanOverexposed, levels: int = 1, out=None, dtype=None):
+        """Batched, device-resident getImage (+ pyramid): frames uint8 CUDA tensor [n, H*W]; levels of `dtype` (torch.float32 (default),
+        torch.float16 or torch.uint8)."""
         import torch
+        _out_type(dtype)
         n = frames.shape[0]
         if out is None:
-            out = [torch.empty((n, w * h), dtype=torch.float32, device=frames.device) for (w, h) in self.level_shapes(rectify, levels)]
-        self.ctx.prepare_batch(frames, _flags(rectify, removeGamma, removeVignette, nanOverexposed), out)
+            tdt = getattr(torch, _dtype_name(dtype))
+            out = [torch.empty((n, w * h), dtype=tdt, device=frames.device) for (w, h) in self.level_shapes(rectify, levels)]
+        self.ctx.prepare_batch(frames, _flags(rectify, removeGamma, removeVignette, nanOverexposed), out, dtype=dtype)
         return out
 
 

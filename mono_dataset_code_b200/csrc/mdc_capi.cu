@@ -97,11 +97,12 @@ struct mdc_ctx {
     cudaStream_t stream = nullptr;
     cudaStream_t pipe_stream[kHostPipeDepth] = {nullptr, nullptr, nullptr};
     uint8_t* pipe_in[kHostPipeDepth] = {nullptr, nullptr, nullptr};
-    float* pipe_out[kHostPipeDepth] = {nullptr, nullptr, nullptr};
+    uint8_t* pipe_out[kHostPipeDepth] = {nullptr, nullptr, nullptr};   // the levels of a chunk (any output type), then its fp32 scratch
     size_t pipe_in_bytes = 0, pipe_out_bytes = 0;
     // scratch for the single-op host entry points
     void* scratch_a = nullptr; size_t scratch_a_bytes = 0;
     void* scratch_b = nullptr; size_t scratch_b_bytes = 0;
+    cudaMemPool_t f32_pool = nullptr;   // narrow output types: fp32 copies of the levels K2 reads, allocated per call (stream-ordered)
     double* d_rc = nullptr;      // responseCalib scratch: gsum[256] gnum[256] factor[1] acc[2] partials[2*kRmsePartialPairs] | fixed-point G-step accumulators (kRcFxOffset)
     long long launches = 0;
 };
@@ -424,15 +425,52 @@ UnmapFlags sanitise(const mdc_ctx* c, unsigned flags) {
     return u;
 }
 
+// The level buffers of one call: the caller's, of element type `type` (MDC_OUT_*), and for a narrow type the fp32 copies of the
+// levels a K2 pass reads (f32[l]; nullptr where no pass reads level l).  px[l] = pixels per frame of level l.
+struct Outs {
+    int type = MDC_OUT_F32;
+    void* lv[MDC_MAX_PYR_LEVELS] = {};
+    float* f32[MDC_MAX_PYR_LEVELS] = {};
+    size_t px[MDC_MAX_PYR_LEVELS] = {};
+    // fp32 source of a K2 pass that reads level l
+    const float* src(int l) const { return type == MDC_OUT_F32 ? static_cast<const float*>(lv[l]) : f32[l]; }
+    // the same levels from frame f0 on
+    Outs from(size_t f0) const {
+        Outs o = *this;
+        for (int l = 0; l < MDC_MAX_PYR_LEVELS; ++l) {
+            if (lv[l]) o.lv[l] = static_cast<uint8_t*>(lv[l]) + f0 * px[l] * mdc_out_elem_size(type);
+            if (f32[l]) o.f32[l] = f32[l] + f0 * px[l];
+        }
+        return o;
+    }
+};
+Outs f32_outs(float* const* levels, int n, const mdc_ctx* c) {       // rectified fp32 levels (context-internal callers)
+    Outs o;
+    for (int l = 0; l < n; ++l) { o.lv[l] = levels[l]; o.px[l] = static_cast<size_t>(c->out_w >> l) * (c->out_h >> l); }
+    return o;
+}
+
+// Levels that a K2 pass reads (need[l] = 1), for `levels` levels of which the first `first_k2` come from K1 (rectifying mode: 3,
+// or fewer) or from unmap_kernel (non-rectifying mode: 1).  The K2 chain behind K1 goes two levels per launch, from levels 2, 4, 6;
+// in non-rectifying mode every level is read by the next one.
+void k2_sources(bool rectify, int levels, bool need[MDC_MAX_PYR_LEVELS]) {
+    for (int l = 0; l < MDC_MAX_PYR_LEVELS; ++l) need[l] = false;
+    if (!rectify) {
+        for (int l = 0; l + 1 < levels; ++l) need[l] = true;
+        return;
+    }
+    for (int l = std::min(levels, kInKernelLevels); l < levels; l += 2) need[l - 1] = true;
+}
+
 // levels beyond the fused epilogue: stand-alone K2 chain, two levels per launch where possible
-int run_deep_levels(mdc_ctx* c, int n_frames, float* const* d_out_levels, int in_kernel, int levels, cudaStream_t stream) {
+int run_deep_levels(mdc_ctx* c, int n_frames, const Outs& o, int in_kernel, int levels, cudaStream_t stream) {
     for (int l = in_kernel; l < levels;) {
         const int sw = c->out_w >> (l - 1), sh = c->out_h >> (l - 1);
         if (l + 1 < levels) {
-            CU_CHECK(launch_pyr_down2(d_out_levels[l - 1], sw, sh, d_out_levels[l], d_out_levels[l + 1], n_frames, stream));
+            CU_CHECK(launch_pyr_down2(o.src(l - 1), sw, sh, o.lv[l], o.lv[l + 1], o.type, o.f32[l + 1], n_frames, stream));
             l += 2;
         } else {
-            CU_CHECK(launch_pyr_down(d_out_levels[l - 1], sw, sh, d_out_levels[l], n_frames, stream));
+            CU_CHECK(launch_pyr_down(o.src(l - 1), sw, sh, o.lv[l], o.type, nullptr, n_frames, stream));
             l += 1;
         }
         c->launches++;
@@ -441,7 +479,7 @@ int run_deep_levels(mdc_ctx* c, int n_frames, float* const* d_out_levels, int in
 }
 
 // K1 through the texture-gather loader.  One launch covers up to kMaxTex chunks (= texture objects).
-int run_fused_tex(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frames, int chunk, UnmapFlags u, float* const* d_out_levels, int levels,
+int run_fused_tex(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frames, int chunk, UnmapFlags u, const Outs& outs, int levels,
                   cudaStream_t stream) {
     const std::vector<cudaTextureObject_t>* objs = nullptr;
     int rc = get_textures(c, d_frames, pitch, n_frames, chunk, &objs);
@@ -460,10 +498,12 @@ int run_fused_tex(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frames, 
         p.tiles = c->d_tiles; p.work_counter = nullptr;
         p.tiles_x = c->tiles_x; p.n_tiles = static_cast<int>(c->tiles.size());
         p.levels = in_kernel;
+        const Outs o = outs.from(static_cast<size_t>(f0));
         for (int l = 0; l < in_kernel; ++l) {
             p.lw[l] = c->out_w >> l; p.lh[l] = c->out_h >> l;
-            p.out[l] = d_out_levels[l] ? d_out_levels[l] + static_cast<size_t>(f0) * p.lw[l] * p.lh[l] : nullptr;
+            p.out[l] = o.lv[l];
         }
+        p.level2_f32 = o.f32[2];
         p.lut_gamma = u.gamma; p.use_vig = u.vig; p.kill = u.kill;
         p.chunk_frames = chunk;
         p.tiles_per_cta = c->tex_tiles_per_cta;
@@ -471,10 +511,10 @@ int run_fused_tex(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frames, 
         TexSet texs;
         memset(&texs, 0, sizeof texs);
         for (int k = 0; k < nc; ++k) texs.tex[k] = (*objs)[c0 + k];
-        CU_CHECK(launch_fused_tex(p, texs, nc, min_ctas, c->tex_prefetch != 0, c->k1_study, stream));
+        CU_CHECK(launch_fused_tex(p, texs, nc, min_ctas, c->tex_prefetch != 0, c->k1_study, outs.type, stream));
         c->launches++;
     }
-    return run_deep_levels(c, n_frames, d_out_levels, in_kernel, levels, stream);
+    return run_deep_levels(c, n_frames, outs, in_kernel, levels, stream);
 }
 
 // What "auto" resolves to (order measured on H100 at 1280x1024: TMA ahead of hybrid and texture gather, DESIGN.md §7); a loader that turns out unusable for a particular
@@ -489,7 +529,7 @@ int auto_loader(const mdc_ctx* c, const uint8_t* frames, int pitch) {
 
 // K1 through the staged loaders (TMA ring or LDG double buffer), levels 0..in_kernel-1 only.  cap_per_sm > 0 bounds the persistent
 // grid (hybrid mode leaves room for the texture kernel's CTAs on every SM).
-int run_fused_staged(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frames, UnmapFlags u, float* const* d_out_levels, int in_kernel,
+int run_fused_staged(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frames, UnmapFlags u, const Outs& outs, int in_kernel,
                      cudaStream_t stream, int loader, int cap_per_sm) {
     FusedParams p;
     memset(&p, 0, sizeof p);
@@ -501,8 +541,9 @@ int run_fused_staged(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frame
     CU_CHECK(cudaMemsetAsync(p.work_counter, 0, sizeof(int), stream));
     p.tiles_x = c->tiles_x; p.n_tiles = static_cast<int>(c->tiles.size());
     p.levels = in_kernel;
-    for (int l = 0; l < in_kernel; ++l) { p.out[l] = d_out_levels[l]; p.lw[l] = c->out_w >> l; p.lh[l] = c->out_h >> l; }
+    for (int l = 0; l < in_kernel; ++l) { p.out[l] = outs.lv[l]; p.lw[l] = c->out_w >> l; p.lh[l] = c->out_h >> l; }
     for (int l = in_kernel; l < MDC_MAX_PYR_LEVELS; ++l) { p.lw[l] = p.lh[l] = 0; }
+    p.level2_f32 = outs.f32[2];
     p.lut_gamma = u.gamma; p.use_vig = u.vig; p.kill = u.kill;
     p.box_px_max = c->box_px_max;
     p.carveout = c->carveout;
@@ -519,14 +560,15 @@ int run_fused_staged(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frame
     // spill-free at 2 CTAs/SM (96 registers) with a deeper ring.
     const int min_ctas = cap_per_sm > 0 ? 3 : c->ctas_per_sm > 0 ? (c->ctas_per_sm <= 2 ? 2 : 3) : (in_kernel > 1 ? 2 : 3);
     p.tma_stages = c->tma_stages > 0 ? std::min(std::max(c->tma_stages, 2), kMaxStages) : fused_tma_stages(p.box_px_max, min_ctas);
-    int per_sm = fused_max_ctas_per_sm(p.box_px_max, tma ? p.tma_stages : kLdgStages, tma, u.vig, in_kernel > 1, min_ctas);
+    int per_sm = fused_max_ctas_per_sm(p.box_px_max, tma ? p.tma_stages : kLdgStages, tma, u.vig, in_kernel > 1, min_ctas, outs.type);
     if (per_sm < 1) { mdc_set_error("fused kernel does not fit on an SM (box %d px)", p.box_px_max); return MDC_ERR_CUDA; }
     if (c->ctas_per_sm > 0) per_sm = std::min(per_sm, c->ctas_per_sm);
     if (cap_per_sm > 0) per_sm = std::min(per_sm, cap_per_sm);
     const long long items = static_cast<long long>(p.n_tiles) * ((n_frames + p.chunk_frames - 1) / p.chunk_frames);
     int grid = static_cast<int>(std::min<long long>(static_cast<long long>(per_sm) * c->sm_count, std::max<long long>(items, 1)));
-    if (c->k1_study != kStudyAll && tma && u.vig && in_kernel == 1 && min_ctas == 3) CU_CHECK(launch_fused_study(p, maps, grid, c->k1_study, stream));
-    else CU_CHECK(launch_fused(p, maps, grid, min_ctas, stream));
+    if (c->k1_study != kStudyAll && tma && u.vig && in_kernel == 1 && min_ctas == 3 && outs.type == MDC_OUT_F32)
+        CU_CHECK(launch_fused_study(p, maps, grid, c->k1_study, stream));
+    else CU_CHECK(launch_fused(p, maps, grid, min_ctas, outs.type, stream));
     c->launches++;
     return MDC_OK;
 }
@@ -536,7 +578,7 @@ int run_fused_staged(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frame
 // the register / shared-memory space that is left.  The idea is that the two pipes add up; on H100 it is
 // slower than the TMA kernel alone (DESIGN.md §7), so `auto` picks it only on request (MDC_AUTO_HYBRID).
 // The leading whole chunks go to the texture kernel, the rest to the staged kernel; fork/join with events around an auxiliary stream.
-int run_fused_hybrid(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frames, int chunk, UnmapFlags u, float* const* d_out_levels, int levels,
+int run_fused_hybrid(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frames, int chunk, UnmapFlags u, const Outs& outs, int levels,
                      cudaStream_t stream) {
     const int in_kernel = std::min(levels, kInKernelLevels);
     const int n_chunks = (n_frames + chunk - 1) / chunk;
@@ -544,32 +586,30 @@ int run_fused_hybrid(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frame
     tex_chunks = std::max(0, std::min(tex_chunks, n_chunks));
     const int n_tex = std::min(n_frames, tex_chunks * chunk), n_stg = n_frames - n_tex;
     if (n_tex == 0 || n_stg == 0 || !tma_pitch_ok(c, d_frames, pitch)) {
-        if (n_stg == 0) return run_fused_tex(c, d_frames, pitch, n_frames, chunk, u, d_out_levels, levels, stream);
-        int rc = run_fused_staged(c, d_frames, pitch, n_frames, u, d_out_levels, in_kernel, stream, -1, 0);
-        return rc != MDC_OK ? rc : run_deep_levels(c, n_frames, d_out_levels, in_kernel, levels, stream);
+        if (n_stg == 0) return run_fused_tex(c, d_frames, pitch, n_frames, chunk, u, outs, levels, stream);
+        int rc = run_fused_staged(c, d_frames, pitch, n_frames, u, outs, in_kernel, stream, -1, 0);
+        return rc != MDC_OK ? rc : run_deep_levels(c, n_frames, outs, in_kernel, levels, stream);
     }
     if (!c->aux_stream) {
         CU_CHECK(cudaStreamCreateWithFlags(&c->aux_stream, cudaStreamNonBlocking));
         CU_CHECK(cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming));
         CU_CHECK(cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming));
     }
-    float* stg_out[MDC_MAX_PYR_LEVELS] = {};
-    for (int l = 0; l < in_kernel; ++l)
-        stg_out[l] = d_out_levels[l] ? d_out_levels[l] + static_cast<size_t>(n_tex) * (c->out_w >> l) * (c->out_h >> l) : nullptr;
+    const Outs stg_out = outs.from(static_cast<size_t>(n_tex));
     CU_CHECK(cudaEventRecord(c->ev_fork, stream));
     CU_CHECK(cudaStreamWaitEvent(c->aux_stream, c->ev_fork, 0));
     // staged kernel first: its persistent CTAs take their slots on every SM, the texture kernel's short CTAs fill what is left
     int rc = run_fused_staged(c, d_frames + static_cast<size_t>(n_tex) * pitch * c->in_h, pitch, n_stg, u, stg_out, in_kernel, stream, 1, c->hyb_stg_ctas);
     if (rc != MDC_OK) return rc;
-    rc = run_fused_tex(c, d_frames, pitch, n_tex, chunk, u, d_out_levels, in_kernel, c->aux_stream);
+    rc = run_fused_tex(c, d_frames, pitch, n_tex, chunk, u, outs, in_kernel, c->aux_stream);
     if (rc != MDC_OK) return rc;
     CU_CHECK(cudaEventRecord(c->ev_join, c->aux_stream));
     CU_CHECK(cudaStreamWaitEvent(stream, c->ev_join, 0));
-    return run_deep_levels(c, n_frames, d_out_levels, in_kernel, levels, stream);
+    return run_deep_levels(c, n_frames, outs, in_kernel, levels, stream);
 }
 
 // loader: -1 = the context's setting (auto: see mdc_ctx_configure); pitch = bytes between input rows (0 = tightly packed)
-int run_fused(mdc_ctx* c, const uint8_t* d_frames, int n_frames, UnmapFlags u, float* const* d_out_levels, int levels,
+int run_fused(mdc_ctx* c, const uint8_t* d_frames, int n_frames, UnmapFlags u, const Outs& outs, int levels,
               cudaStream_t stream, int loader = -1, int pitch = 0) {
     if (pitch <= 0) pitch = c->in_w;
     if (loader < 0) loader = c->use_tma;
@@ -581,15 +621,15 @@ int run_fused(mdc_ctx* c, const uint8_t* d_frames, int n_frames, UnmapFlags u, f
         }
         const int chunk = tex_chunk_frames(c, d_frames, pitch, c->chunk_frames > 0 ? c->chunk_frames : 48);
         if (chunk > 0) {
-            if (loader == 3) return run_fused_hybrid(c, d_frames, pitch, n_frames, chunk, u, d_out_levels, levels, stream);
-            return run_fused_tex(c, d_frames, pitch, n_frames, chunk, u, d_out_levels, levels, stream);
+            if (loader == 3) return run_fused_hybrid(c, d_frames, pitch, n_frames, chunk, u, outs, levels, stream);
+            return run_fused_tex(c, d_frames, pitch, n_frames, chunk, u, outs, levels, stream);
         }
         if (c->use_tma >= 2) { mdc_set_error("texture-gather loader requested but unusable for this geometry/pointer"); return MDC_ERR_UNSUPPORTED; }
         loader = tma_pitch_ok(c, d_frames, pitch) ? 1 : 0;      // auto: this pointer / batch cannot go through textures
     }
     const int in_kernel = std::min(levels, kInKernelLevels);
-    int rc = run_fused_staged(c, d_frames, pitch, n_frames, u, d_out_levels, in_kernel, stream, loader, 0);
-    return rc != MDC_OK ? rc : run_deep_levels(c, n_frames, d_out_levels, in_kernel, levels, stream);
+    int rc = run_fused_staged(c, d_frames, pitch, n_frames, u, outs, in_kernel, stream, loader, 0);
+    return rc != MDC_OK ? rc : run_deep_levels(c, n_frames, outs, in_kernel, levels, stream);
 }
 
 // Self-check of the texture-gather loader, run once per context: K1 over three synthetic frames (all byte values, saturated
@@ -631,9 +671,9 @@ void tex_selfcheck(mdc_ctx* c) {
     const int study0 = c->k1_study, use_tma0 = c->use_tma;
     c->k1_study = kStudyAll;             // the floor-study variants compute garbage by design
     c->use_tma = -1;                     // MDC_USE_TMA=2/3 would refuse the texture loader while tex_ok is still false
-    ok = ok && run_fused(c, frames, nf, u, la, 1, c->stream, 2, pitch) == MDC_OK;
+    ok = ok && run_fused(c, frames, nf, u, f32_outs(la, 1, c), 1, c->stream, 2, pitch) == MDC_OK;
     const bool tma_ref = tma_pitch_ok(c, frames, pitch);
-    ok = ok && run_fused(c, frames, nf, u, lb, 1, c->stream, tma_ref ? 1 : 0, pitch) == MDC_OK;
+    ok = ok && run_fused(c, frames, nf, u, f32_outs(lb, 1, c), 1, c->stream, tma_ref ? 1 : 0, pitch) == MDC_OK;
     c->k1_study = study0;
     c->use_tma = use_tma0;
     ok = ok && launch_count_mismatch(out_a, out_b, nf * n_out, d_bad, c->stream) == cudaSuccess;
@@ -761,6 +801,7 @@ extern "C" void mdc_ctx_destroy(mdc_ctx* c) {
         cudaFree(c->pipe_in[s]); cudaFree(c->pipe_out[s]);
     }
     cudaFree(c->scratch_a); cudaFree(c->scratch_b);
+    if (c->f32_pool) cudaMemPoolDestroy(c->f32_pool);
     if (c->stream) cudaStreamDestroy(c->stream);
     delete c;
 }
@@ -824,7 +865,8 @@ extern "C" int mdc_unmap_u8(mdc_ctx* c, const uint8_t* d_in, float* d_out, int n
     CU_CHECK(cudaSetDevice(c->device));
     const UnmapFlags u = sanitise(c, flags);
     cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
-    CU_CHECK(launch_unmap(d_in, d_out, static_cast<size_t>(n), n_frames, u.gamma ? c->d_ginv : nullptr, u.vig ? c->d_vinv : nullptr, u.kill, s));
+    CU_CHECK(launch_unmap(d_in, d_out, MDC_OUT_F32, nullptr, static_cast<size_t>(n), n_frames, u.gamma ? c->d_ginv : nullptr,
+                          u.vig ? c->d_vinv : nullptr, u.kill, s));
     c->launches++;
     return finish(c, stream, s);
 }
@@ -852,7 +894,7 @@ extern "C" int mdc_undistort_u8(mdc_ctx* c, const uint8_t* d_in, float* d_out, i
     CU_CHECK(cudaSetDevice(c->device));
     cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
     float* lv[1] = {d_out};
-    rc = run_fused(c, d_in, n_frames, UnmapFlags{false, false, false}, lv, 1, s);
+    rc = run_fused(c, d_in, n_frames, UnmapFlags{false, false, false}, f32_outs(lv, 1, c), 1, s);
     if (rc != MDC_OK) return rc;
     return finish(c, stream, s);
 }
@@ -872,17 +914,25 @@ extern "C" int mdc_pyr_down(mdc_ctx* c, const float* d_src, int src_w, int src_h
     if (!c || !d_src || !d_dst || src_w < 0 || src_h < 0 || n_frames < 0) { mdc_set_error("mdc_pyr_down: bad argument"); return MDC_ERR_INVALID_ARG; }
     CU_CHECK(cudaSetDevice(c->device));
     cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
-    CU_CHECK(launch_pyr_down(d_src, src_w, src_h, d_dst, n_frames, s));
+    CU_CHECK(launch_pyr_down(d_src, src_w, src_h, d_dst, MDC_OUT_F32, nullptr, n_frames, s));
     c->launches++;
     return finish(c, stream, s);
 }
 
-static int prepare_batch_impl(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frames, unsigned flags,
-                              float* const* d_out_levels, int levels, mdc_stream stream);
+// scratch: device memory for the fp32 copies of the levels a K2 pass reads (narrow output types only), at least
+// prepare_f32_scratch_bytes(...) bytes, or nullptr to allocate it from the context's pool on the call's stream.
+static int prepare_batch_impl(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frames, unsigned flags, int out_type,
+                              void* const* d_out_levels, int levels, mdc_stream stream, void* scratch = nullptr);
+
+int mdc_check_out_type(int out_type, const char* where) {
+    if (out_type == MDC_OUT_F32 || out_type == MDC_OUT_F16 || out_type == MDC_OUT_U8) return MDC_OK;
+    mdc_set_error("%s: unknown output type %d", where, out_type);
+    return MDC_ERR_INVALID_ARG;
+}
 
 extern "C" int mdc_prepare_batch(mdc_ctx* c, const uint8_t* d_frames, int n_frames, unsigned flags,
                                  float* const* d_out_levels, int levels, mdc_stream stream) {
-    return prepare_batch_impl(c, d_frames, 0, n_frames, flags, d_out_levels, levels, stream);
+    return prepare_batch_impl(c, d_frames, 0, n_frames, flags, MDC_OUT_F32, reinterpret_cast<void* const*>(d_out_levels), levels, stream);
 }
 
 extern "C" int mdc_prepare_batch_pitched(mdc_ctx* c, const uint8_t* d_frames, size_t row_pitch_bytes, int n_frames, unsigned flags,
@@ -891,43 +941,112 @@ extern "C" int mdc_prepare_batch_pitched(mdc_ctx* c, const uint8_t* d_frames, si
         mdc_set_error("mdc_prepare_batch_pitched: row pitch %zu for %d-pixel rows", row_pitch_bytes, c->in_w);
         return MDC_ERR_INVALID_ARG;
     }
-    return prepare_batch_impl(c, d_frames, static_cast<int>(row_pitch_bytes), n_frames, flags, d_out_levels, levels, stream);
+    return prepare_batch_impl(c, d_frames, static_cast<int>(row_pitch_bytes), n_frames, flags, MDC_OUT_F32,
+                              reinterpret_cast<void* const*>(d_out_levels), levels, stream);
 }
 
-static int prepare_batch_impl(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frames, unsigned flags,
-                              float* const* d_out_levels, int levels, mdc_stream stream) {
+extern "C" int mdc_prepare_batch_ex(mdc_ctx* c, const uint8_t* d_frames, size_t row_pitch_bytes, int n_frames, unsigned flags, int out_type,
+                                    void* const* d_out_levels, int levels, mdc_stream stream) {
+    int rc = mdc_check_out_type(out_type, "mdc_prepare_batch_ex");
+    if (rc != MDC_OK) return rc;
+    if (c && row_pitch_bytes != 0 && (row_pitch_bytes < static_cast<size_t>(c->in_w) || row_pitch_bytes > (1u << 30))) {
+        mdc_set_error("mdc_prepare_batch_ex: row pitch %zu for %d-pixel rows", row_pitch_bytes, c->in_w);
+        return MDC_ERR_INVALID_ARG;
+    }
+    return prepare_batch_impl(c, d_frames, static_cast<int>(row_pitch_bytes), n_frames, flags, out_type, d_out_levels, levels, stream);
+}
+
+namespace {
+// Bytes of fp32 scratch a narrow-type call needs per frame (0 for MDC_OUT_F32 and wherever no K2 pass runs).
+size_t prepare_f32_scratch_bytes(const mdc_ctx* c, bool rectify, int out_type, int levels) {
+    if (out_type == MDC_OUT_F32) return 0;
+    bool need[MDC_MAX_PYR_LEVELS];
+    k2_sources(rectify, levels, need);
+    size_t b = 0;
+    for (int l = 0; l < levels; ++l)
+        if (need[l]) b += ((static_cast<size_t>((rectify ? c->out_w : c->in_w) >> l) * ((rectify ? c->out_h : c->in_h) >> l) * 4 + 15) & ~size_t(15));
+    return b;
+}
+int f32_pool(mdc_ctx* c, cudaMemPool_t* out) {
+    if (!c->f32_pool) {     // a pool of the context's own, kept warm between calls (the release threshold keeps its memory mapped)
+        cudaMemPoolProps props = {};
+        props.allocType = cudaMemAllocationTypePinned;
+        props.location.type = cudaMemLocationTypeDevice;
+        props.location.id = c->device;
+        CU_CHECK(cudaMemPoolCreate(&c->f32_pool, &props));
+        uint64_t keep = ~0ull;
+        CU_CHECK(cudaMemPoolSetAttribute(c->f32_pool, cudaMemPoolAttrReleaseThreshold, &keep));
+    }
+    *out = c->f32_pool;
+    return MDC_OK;
+}
+}  // namespace
+
+static int prepare_batch_impl(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frames, unsigned flags, int out_type,
+                              void* const* d_out_levels, int levels, mdc_stream stream, void* scratch) {
     if (!c || !d_frames || !d_out_levels || n_frames < 0 || levels < 1 || levels > MDC_MAX_PYR_LEVELS) {
         mdc_set_error("mdc_prepare_batch: bad argument");
         return MDC_ERR_INVALID_ARG;
     }
     if (c->in_w < 1) { mdc_set_error("mdc_prepare_batch: context has no image geometry"); return MDC_ERR_INVALID_OBJECT; }
     const bool rectify = (flags & MDC_RECTIFY) != 0;
+    Outs o;
+    o.type = out_type;
     for (int l = 0; l < levels; ++l) {   // a level that has no pixels (tiny images) may legitimately be a NULL buffer
         const int lw = (rectify ? c->out_w : c->in_w) >> l, lh = (rectify ? c->out_h : c->in_h) >> l;
         if (!d_out_levels[l] && lw > 0 && lh > 0) { mdc_set_error("mdc_prepare_batch: output level %d is NULL", l); return MDC_ERR_INVALID_ARG; }
+        o.lv[l] = d_out_levels[l];
+        o.px[l] = static_cast<size_t>(lw) * lh;
     }
     if (rectify && !c->have_fov) { mdc_set_error("getImage(rectify) on an invalid rectifier"); return MDC_ERR_INVALID_OBJECT; }
     if (n_frames == 0) return MDC_OK;
     CU_CHECK(cudaSetDevice(c->device));
     cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
+    // narrow output types: the levels a K2 pass reads are also written in fp32, to scratch, and K2 reads those
+    const size_t f32_bytes = prepare_f32_scratch_bytes(c, rectify, out_type, levels) * static_cast<size_t>(n_frames);
+    void* pooled = nullptr;
+    if (f32_bytes > 0) {
+        if (!scratch) {
+            cudaMemPool_t pool;
+            int rc = f32_pool(c, &pool);
+            if (rc != MDC_OK) return rc;
+            CU_CHECK(cudaMallocFromPoolAsync(&pooled, f32_bytes, pool, s));
+            scratch = pooled;
+        }
+        bool need[MDC_MAX_PYR_LEVELS];
+        k2_sources(rectify, levels, need);
+        uint8_t* at = static_cast<uint8_t*>(scratch);
+        for (int l = 0; l < levels; ++l)
+            if (need[l]) { o.f32[l] = reinterpret_cast<float*>(at); at += ((o.px[l] * 4 + 15) & ~size_t(15)) * n_frames; }
+    }
+    int rc = MDC_OK;
     // mode switch of DatasetReader::getImage, BenchmarkDatasetReader.h:210-241
     const bool photometric = (flags & (MDC_REMOVE_GAMMA | MDC_REMOVE_VIGNETTE | MDC_NAN_OVEREXPOSED)) != 0;
     UnmapFlags u{false, false, false};
     if (photometric) u = sanitise(c, flags);
     if (rectify) {
-        int rc = run_fused(c, d_frames, n_frames, u, d_out_levels, levels, s, -1, pitch);
-        if (rc != MDC_OK) return rc;
+        rc = run_fused(c, d_frames, n_frames, u, o, levels, s, -1, pitch);
+    } else if (pitch > 0 && pitch != c->in_w) {
+        mdc_set_error("padded rows are supported in rectifying mode only");
+        rc = MDC_ERR_UNSUPPORTED;
     } else {
-        if (pitch > 0 && pitch != c->in_w) { mdc_set_error("padded rows are supported in rectifying mode only"); return MDC_ERR_UNSUPPORTED; }
-        const size_t n = static_cast<size_t>(c->in_w) * c->in_h;
-        CU_CHECK(launch_unmap(d_frames, d_out_levels[0], n, n_frames, u.gamma ? c->d_ginv : nullptr, u.vig ? c->d_vinv : nullptr, u.kill, s));
-        c->launches++;
-        for (int l = 1; l < levels; ++l) {
-            CU_CHECK(launch_pyr_down(d_out_levels[l - 1], c->in_w >> (l - 1), c->in_h >> (l - 1), d_out_levels[l], n_frames, s));
+        rc = [&]() -> int {
+            const size_t n = static_cast<size_t>(c->in_w) * c->in_h;
+            CU_CHECK(launch_unmap(d_frames, o.lv[0], o.type, o.f32[0], n, n_frames, u.gamma ? c->d_ginv : nullptr, u.vig ? c->d_vinv : nullptr,
+                                  u.kill, s));
             c->launches++;
-        }
+            for (int l = 1; l < levels; ++l) {
+                CU_CHECK(launch_pyr_down(o.src(l - 1), c->in_w >> (l - 1), c->in_h >> (l - 1), o.lv[l], o.type, o.f32[l], n_frames, s));
+                c->launches++;
+            }
+            return MDC_OK;
+        }();
     }
-    return finish(c, stream, s);
+    if (pooled) {
+        const cudaError_t e = cudaFreeAsync(pooled, s);      // stream-ordered: after the launches above
+        if (rc == MDC_OK && e != cudaSuccess) { mdc_set_error("cudaFreeAsync failed: %s", cudaGetErrorString(e)); rc = MDC_ERR_CUDA; }
+    }
+    return rc != MDC_OK ? rc : finish(c, stream, s);
 }
 
 extern "C" int mdc_fov_distort_coordinates_device(const mdc_fov* f, float* d_x, float* d_y, size_t n, int device, mdc_stream stream) {
@@ -1254,6 +1373,20 @@ extern "C" int mdc_undistort_f32_host(mdc_ctx* c, const float* in, float* out, i
 
 extern "C" int mdc_prepare_batch_host(mdc_ctx* c, const uint8_t* frames, int n_frames, unsigned flags,
                                       float* const* out_levels, int levels) {
+    return mdc_prepare_batch_host_ex(c, frames, n_frames, flags, MDC_OUT_F32, reinterpret_cast<void* const*>(out_levels), levels);
+}
+
+extern "C" int mdc_seq_prepare_ex(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned flags, int out_type, void* const* h_out_levels,
+                                  int levels, int threads) {
+    const int rc = mdc_check_out_type(out_type, "mdc_seq_prepare");
+    if (rc != MDC_OK) return rc;
+    return mdc_seq_prepare_feed(c, s, first, count, flags, out_type, h_out_levels, levels, threads, mdc_prepare_batch_host_ex);
+}
+
+extern "C" int mdc_prepare_batch_host_ex(mdc_ctx* c, const uint8_t* frames, int n_frames, unsigned flags, int out_type,
+                                         void* const* out_levels, int levels) {
+    int rc0 = mdc_check_out_type(out_type, "mdc_prepare_batch_host_ex");
+    if (rc0 != MDC_OK) return rc0;
     if (!c || !frames || !out_levels || n_frames < 0 || levels < 1 || levels > MDC_MAX_PYR_LEVELS) {
         mdc_set_error("mdc_prepare_batch_host: bad argument");
         return MDC_ERR_INVALID_ARG;
@@ -1279,7 +1412,11 @@ extern "C" int mdc_prepare_batch_host(mdc_ctx* c, const uint8_t* frames, int n_f
     // Rows that are not a multiple of 16 bytes cannot be described to TMA — but the H2D copy can pad them for free (2-D copy into a
     // device buffer with a 32-byte multiple pitch), which keeps such widths on the fast loaders instead of the 2x slower LDG one.
     const int pitch = (rectify && c->in_w % 16 != 0 && c->plan_tma_ok) ? ((c->in_w + 31) & ~31) : c->in_w;
-    const size_t in_bytes = static_cast<size_t>(chunk) * pitch * c->in_h, out_bytes = static_cast<size_t>(chunk) * px_per_frame * 4;
+    // pipe buffers and D2H copies in the output type's element size; a narrow type's fp32 scratch (levels K2 reads) follows the levels
+    const size_t esize = mdc_out_elem_size(out_type);
+    const size_t lv_bytes = (static_cast<size_t>(chunk) * px_per_frame * esize + 255) & ~size_t(255);
+    const size_t in_bytes = static_cast<size_t>(chunk) * pitch * c->in_h,
+                 out_bytes = lv_bytes + static_cast<size_t>(chunk) * prepare_f32_scratch_bytes(c, rectify, out_type, levels);
     if (c->pipe_in_bytes < in_bytes || c->pipe_out_bytes < out_bytes) {
         for (int s = 0; s < kHostPipeDepth; ++s) {
             if (c->pipe_stream[s]) cudaStreamSynchronize(c->pipe_stream[s]);
@@ -1311,12 +1448,14 @@ extern "C" int mdc_prepare_batch_host(mdc_ctx* c, const uint8_t* frames, int n_f
             ? cudaMemcpyAsync(c->pipe_in[s], frames + static_cast<size_t>(f0) * n_in, static_cast<size_t>(nf) * n_in, cudaMemcpyHostToDevice, st)
             : cudaMemcpy2DAsync(c->pipe_in[s], static_cast<size_t>(pitch), frames + static_cast<size_t>(f0) * n_in, static_cast<size_t>(c->in_w),
                                 static_cast<size_t>(c->in_w), static_cast<size_t>(c->in_h) * nf, cudaMemcpyHostToDevice, st);
-        float* lv[MDC_MAX_PYR_LEVELS];
+        void* lv[MDC_MAX_PYR_LEVELS];
         size_t off = 0;
-        for (int l = 0; l < levels; ++l) { lv[l] = c->pipe_out[s] + off; off += static_cast<size_t>(nf) * lvl_px[l]; }
-        if (ce == cudaSuccess) rc = prepare_batch_impl(c, c->pipe_in[s], pitch == c->in_w ? 0 : pitch, nf, flags, lv, levels, st);
+        for (int l = 0; l < levels; ++l) { lv[l] = c->pipe_out[s] + off; off += static_cast<size_t>(nf) * lvl_px[l] * esize; }
+        if (ce == cudaSuccess)
+            rc = prepare_batch_impl(c, c->pipe_in[s], pitch == c->in_w ? 0 : pitch, nf, flags, out_type, lv, levels, st, c->pipe_out[s] + lv_bytes);
         for (int l = 0; l < levels && rc == MDC_OK && ce == cudaSuccess; ++l)
-            ce = cudaMemcpyAsync(out_levels[l] + static_cast<size_t>(f0) * lvl_px[l], lv[l], static_cast<size_t>(nf) * lvl_px[l] * 4, cudaMemcpyDeviceToHost, st);
+            ce = cudaMemcpyAsync(static_cast<uint8_t*>(out_levels[l]) + static_cast<size_t>(f0) * lvl_px[l] * esize, lv[l],
+                                 static_cast<size_t>(nf) * lvl_px[l] * esize, cudaMemcpyDeviceToHost, st);
         if (ce != cudaSuccess) { mdc_set_error("mdc_prepare_batch_host: copy failed: %s", cudaGetErrorString(ce)); rc = MDC_ERR_CUDA; }
     }
     const cudaError_t drained = drain();

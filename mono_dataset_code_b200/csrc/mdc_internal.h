@@ -10,6 +10,11 @@
 // Thread-local error message behind mdc_last_error().
 void mdc_set_error(const char* fmt, ...);
 
+// Output types of the prepare calls (MDC_OUT_*): element size, and the check every _ex entry point makes first (no device needed):
+// MDC_OK, or MDC_ERR_INVALID_ARG with "<where>: unknown output type <t>".
+inline size_t mdc_out_elem_size(int out_type) { return out_type == MDC_OUT_F16 ? 2 : out_type == MDC_OUT_U8 ? 1 : 4; }
+int mdc_check_out_type(int out_type, const char* where);
+
 // Host-side state of the FOV rectifier (the members of the reference's UndistorterFOV,
 // FOVUndistorter.h:85-95, plus bookkeeping).
 struct mdc_fov {
@@ -63,4 +68,10 @@ struct mdc_seq_feed_stage { void* pinned[2] = {nullptr, nullptr}; size_t bytes[2
 bool mdc_seq_read_file(const mdc_seq* s, int id, std::vector<uint8_t>* file);      // frame id's file bytes (folder file or zip entry)
 std::mutex& mdc_seq_feed_mutex(const mdc_seq* s);                                   // one feed at a time per sequence object
 mdc_seq_feed_stage* mdc_seq_device_stage(const mdc_seq* s);
+// The decode-ahead host feed behind mdc_seq_prepare and mdc_seq_prepare_ex (mdc_sequence.cpp).  Each decoded chunk goes to `prepare`
+// (mdc_prepare_batch_host_ex's signature), so that the sequence reader calls nothing of the GPU side but what its caller hands it.
+typedef int (*mdc_host_prepare_fn)(mdc_ctx* c, const uint8_t* frames, int n_frames, unsigned flags, int out_type, void* const* out_levels,
+                                   int levels);
+int mdc_seq_prepare_feed(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned flags, int out_type, void* const* h_out_levels,
+                         int levels, int threads, mdc_host_prepare_fn prepare);
 int mdc_seq_default_threads();                                                      // threads = 0 of the feeds

@@ -585,6 +585,12 @@ int run_device_feed(const mdc_seq* s, const int* ids, int count, int w, int h, i
 
 extern "C" int mdc_seq_prepare_device(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned flags, float* const* d_out_levels, int levels,
                                       int threads, mdc_stream stream) {
+    return mdc_seq_prepare_device_ex(c, s, first, count, flags, MDC_OUT_F32, reinterpret_cast<void* const*>(d_out_levels), levels, threads, stream);
+}
+
+extern "C" int mdc_seq_prepare_device_ex(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned flags, int out_type,
+                                         void* const* d_out_levels, int levels, int threads, mdc_stream stream) {
+    if (mdc_check_out_type(out_type, "mdc_seq_prepare_device") != MDC_OK) return MDC_ERR_INVALID_ARG;
     // the argument checks of mdc_seq_prepare, in the same order
     if (!s || !d_out_levels) { mdc_set_error("mdc_seq_prepare_device: bad argument"); return MDC_ERR_INVALID_ARG; }
     const int n_files = mdc_seq_num_images(s);
@@ -622,9 +628,11 @@ extern "C" int mdc_seq_prepare_device(mdc_ctx* c, const mdc_seq* s, int first, i
     auto prepare = [&](const FeedChunk& fc) -> int {
         for (int i = 0; i < fc.n; ++i)
             if (fc.status[static_cast<size_t>(i)] != MDC_OK) { fail_msg = fc.msg[static_cast<size_t>(i)]; return MDC_ERR_FORMAT; }
-        std::vector<float*> outs(static_cast<size_t>(levels));
-        for (int l = 0; l < levels; ++l) outs[static_cast<size_t>(l)] = d_out_levels[l] ? d_out_levels[l] + static_cast<size_t>(fc.f0) * level_px[static_cast<size_t>(l)] : nullptr;
-        return mdc_prepare_batch_pitched(c, fc.frames, pitch, fc.n, flags, outs.data(), levels, st);
+        std::vector<void*> outs(static_cast<size_t>(levels));
+        const size_t esize = mdc_out_elem_size(out_type);
+        for (int l = 0; l < levels; ++l)
+            outs[static_cast<size_t>(l)] = d_out_levels[l] ? static_cast<uint8_t*>(d_out_levels[l]) + static_cast<size_t>(fc.f0) * level_px[static_cast<size_t>(l)] * esize : nullptr;
+        return mdc_prepare_batch_ex(c, fc.frames, pitch, fc.n, flags, out_type, outs.data(), levels, st);
     };
     const int rc = run_device_feed(s, ids.data(), count, in_w, in_h, threads, nullptr, pitch, st, prepare, "mdc_seq_prepare_device");
     if (rc == MDC_ERR_FORMAT) {

@@ -16,6 +16,7 @@
 //
 // All of this is HBM-bound byte/float streaming; there is no GEMM-shaped work, so no tcgen05.
 #include <cuda.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <float.h>
 #include <stdint.h>
@@ -65,6 +66,34 @@ __device__ __forceinline__ void sts_u32(uint32_t addr, uint32_t v) {
 // evict-first store: the rectified images are written once and never re-read by this kernel; keep L2
 // for the input frames of the current chunk and for the calibration tables.
 __device__ __forceinline__ void stg_cs(float* p, float v) { asm volatile("st.global.cs.f32 [%0], %1;" ::"l"(p), "f"(v) : "memory"); }
+
+// ---- output types (MDC_OUT_*): every level is computed in fp32 and converted only where it is stored
+template <int kOut> struct OutElem { using T = float; };
+template <> struct OutElem<MDC_OUT_F16> { using T = __half; };
+template <> struct OutElem<MDC_OUT_U8> { using T = uint8_t; };
+// cv::saturate_cast<uchar>(float), i.e. convertTo(CV_8U), as OpenCV computes it on x86-64: cvRound is cvtss2si (round half to even;
+// NaN, +-inf and values outside int32 give INT_MIN), then the clamp to [0, 255].  cvt.rni saturates instead (NaN -> 0, large -> INT_MAX),
+// so what x86 turns into INT_MIN at the top end is mapped to 0 explicitly.
+__device__ __forceinline__ uint32_t conv_u8(float v) {
+    int r = __float2int_rn(v);
+    if (!(v < 2147483648.0f)) r = 0;              // NaN, +inf, >= 2^31
+    return static_cast<uint32_t>(min(max(r, 0), 255));
+}
+__device__ __forceinline__ void stg_cs(__half* p, float v) {
+    asm volatile("st.global.cs.b16 [%0], %1;" ::"l"(p), "h"(__half_as_ushort(__float2half_rn(v))) : "memory");
+}
+__device__ __forceinline__ void stg_cs(uint8_t* p, float v) { asm volatile("st.global.cs.u8 [%0], %1;" ::"l"(p), "r"(conv_u8(v)) : "memory"); }
+// plain stores of one / four converted pixels (streaming kernels)
+__device__ __forceinline__ void put(float* p, float v) { *p = v; }
+__device__ __forceinline__ void put(__half* p, float v) { *p = __float2half_rn(v); }
+__device__ __forceinline__ void put(uint8_t* p, float v) { *p = static_cast<uint8_t>(conv_u8(v)); }
+__device__ __forceinline__ void put4(__half* p, float4 o) {
+    const __half2 a = __floats2half2_rn(o.x, o.y), b = __floats2half2_rn(o.z, o.w);
+    *reinterpret_cast<uint2*>(p) = make_uint2(*reinterpret_cast<const uint32_t*>(&a), *reinterpret_cast<const uint32_t*>(&b));
+}
+__device__ __forceinline__ void put4(uint8_t* p, float4 o) {
+    *reinterpret_cast<uint32_t*>(p) = conv_u8(o.x) | conv_u8(o.y) << 8 | conv_u8(o.z) << 16 | conv_u8(o.w) << 24;
+}
 
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
@@ -166,9 +195,14 @@ __device__ __forceinline__ float lut_value(const FusedParams& p, int v) {
     return r;
 }
 
+// kStudy = the floor-study bits | the output type << kOutShift (see k1_variant).  Only the stores depend on the output type; a narrow
+// type also writes the fp32 level 2 to p.level2_f32 when the K2 chain needs it.  The fp32 kernels must keep their machine code, so
+// the output type rides in kStudy (the fp32 instantiations keep their names and template arguments) and is spelled out where it is
+// used: a kernel-local constant here (the frame-loop lambda sees it) changes the fp32 code (scripts/sass_compare.py checks this).
 template <bool kTma, bool kVig, bool kPyr, int kMinCtas, int kStudy = kStudyAll>
 __global__ void __launch_bounds__(kTma ? kConsumers + 32 : kConsumers, kMinCtas)
 fused_prepare_kernel(const __grid_constant__ FusedParams p, const __grid_constant__ TmaMaps maps) {
+    using TOut = typename OutElem<(kStudy >> kOutShift)>::T;
     const int kNs = kTma ? p.tma_stages : kLdgStages;   // ring depth (runtime: as many stages as fit next to 3 CTAs/SM)
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // ---- shared-memory carve-up (see fused_smem_bytes)
@@ -343,23 +377,30 @@ fused_prepare_kernel(const __grid_constant__ FusedParams p, const __grid_constan
                 vi2[h][k] = pack2(vi[2 * h][k], vi[2 * h + 1][k]);
             }
 
-        float* o0 = p.out[0] + static_cast<size_t>(f_begin) * p.lw[0] * p.lh[0] + static_cast<size_t>(oy0) * p.out_w + ox;
+        TOut* o0 = static_cast<TOut*>(p.out[0]) + static_cast<size_t>(f_begin) * p.lw[0] * p.lh[0] + static_cast<size_t>(oy0) * p.out_w + ox;
         const size_t o0_step = static_cast<size_t>(p.lw[0]) * p.lh[0];
         const bool x_ok = ox < p.out_w;
         // pyramid levels 1-2: per-item output pointers and store predicates (advanced by one image per frame)
-        float *o1 = nullptr, *o2 = nullptr;
+        TOut *o1 = nullptr, *o2 = nullptr;
+        float* o2f = nullptr;                // narrow types: fp32 level 2 for the K2 chain
         uint32_t o1_step = 0, o2_step = 0;   // elements per image of level 1 / 2 (< 2^31)
-        bool st1 = false, st2 = false;
+        bool st1 = false, st2 = false, st2f = false;
         if (kPyr) {
             const int X1 = (tx0 >> 1) + (lane >> 1), Y1 = (ty0 >> 1) + 2 * warp + (lane & 1);   // even lane: upper block, odd lane: lower block
             st1 = X1 < p.lw[1] && Y1 < p.lh[1];
             o1_step = static_cast<uint32_t>(p.lw[1]) * static_cast<uint32_t>(p.lh[1]);
-            o1 = p.out[1] + static_cast<size_t>(f_begin) * o1_step + static_cast<size_t>(Y1) * p.lw[1] + X1;
+            o1 = static_cast<TOut*>(p.out[1]) + static_cast<size_t>(f_begin) * o1_step + static_cast<size_t>(Y1) * p.lw[1] + X1;
             if (p.levels > 2) {
                 const int X2 = (tx0 >> 2) + (lane >> 2), Y2 = (ty0 >> 2) + warp;
                 st2 = (lane & 3) == 0 && X2 < p.lw[2] && Y2 < p.lh[2];
                 o2_step = static_cast<uint32_t>(p.lw[2]) * static_cast<uint32_t>(p.lh[2]);
-                o2 = p.out[2] + static_cast<size_t>(f_begin) * o2_step + static_cast<size_t>(Y2) * p.lw[2] + X2;
+                o2 = static_cast<TOut*>(p.out[2]) + static_cast<size_t>(f_begin) * o2_step + static_cast<size_t>(Y2) * p.lw[2] + X2;
+                if constexpr ((kStudy >> kOutShift) != MDC_OUT_F32) {
+                    if (p.level2_f32) {
+                        o2f = p.level2_f32 + static_cast<size_t>(f_begin) * o2_step + static_cast<size_t>(Y2) * p.lw[2] + X2;
+                        st2f = st2;
+                    }
+                }
             }
         }
 
@@ -466,6 +507,10 @@ fused_prepare_kernel(const __grid_constant__ FusedParams p, const __grid_constan
                     const float l2 = __fmul_rn(0.25f, __fadd_rn(__fadd_rn(__fadd_rn(l1, b2), c2), d2));   // lanes = 0 mod 4
                     if (st2) stg_cs(o2, l2);
                     o2 += o2_step;
+                    if constexpr ((kStudy >> kOutShift) != MDC_OUT_F32) {
+                        if (st2f) stg_cs(o2f, l2);
+                        o2f += o2_step;
+                    }
                 }
             }
             if (!kTma && kStaged) {
@@ -476,7 +521,7 @@ fused_prepare_kernel(const __grid_constant__ FusedParams p, const __grid_constan
         };
         if (staged) { if (has_black) run_frames(std::true_type{}, std::true_type{}); else run_frames(std::true_type{}, std::false_type{}); }
         else run_frames(std::false_type{}, std::true_type{});
-        if (!(kStudy & kStudyStores) && study_acc == 0x9e3779b9u && x_ok) stg_cs(p.out[0], 0.0f);   // keeps the folded pixels alive
+        if (!(kStudy & kStudyStores) && study_acc == 0x9e3779b9u && x_ok) stg_cs(static_cast<TOut*>(p.out[0]), 0.0f);   // keeps the folded pixels alive
         if (!kTma) {         // LDG loader: thread 0 pulls the next item for the whole CTA
             consumer_barrier();
             if (tid == 0) s_item[0] = static_cast<int>(gridDim.x) + atomicAdd(p.work_counter, 1);
@@ -503,33 +548,36 @@ int fused_tma_stages(int box_px_max, int ctas_per_sm) {
 }
 
 typedef void (*FusedKernelFn)(const FusedParams, const TmaMaps);
-template <int kMinCtas>
+template <int kMinCtas, int kV = kStudyAll>
 static FusedKernelFn fused_variant_t(bool tma, bool vig, bool pyr) {
     if (tma) {
-        if (vig) return pyr ? fused_prepare_kernel<true, true, true, kMinCtas> : fused_prepare_kernel<true, true, false, kMinCtas>;
-        return pyr ? fused_prepare_kernel<true, false, true, kMinCtas> : fused_prepare_kernel<true, false, false, kMinCtas>;
+        if (vig) return pyr ? fused_prepare_kernel<true, true, true, kMinCtas, kV> : fused_prepare_kernel<true, true, false, kMinCtas, kV>;
+        return pyr ? fused_prepare_kernel<true, false, true, kMinCtas, kV> : fused_prepare_kernel<true, false, false, kMinCtas, kV>;
     }
-    if (vig) return pyr ? fused_prepare_kernel<false, true, true, kMinCtas> : fused_prepare_kernel<false, true, false, kMinCtas>;
-    return pyr ? fused_prepare_kernel<false, false, true, kMinCtas> : fused_prepare_kernel<false, false, false, kMinCtas>;
+    if (vig) return pyr ? fused_prepare_kernel<false, true, true, kMinCtas, kV> : fused_prepare_kernel<false, true, false, kMinCtas, kV>;
+    return pyr ? fused_prepare_kernel<false, false, true, kMinCtas, kV> : fused_prepare_kernel<false, false, false, kMinCtas, kV>;
 }
-static FusedKernelFn fused_variant(bool tma, bool vig, bool pyr, int min_ctas) {
-    return min_ctas <= 2 ? fused_variant_t<2>(tma, vig, pyr) : fused_variant_t<3>(tma, vig, pyr);
+static FusedKernelFn fused_variant(bool tma, bool vig, bool pyr, int min_ctas, int out_type) {
+    constexpr int kF16 = k1_variant(MDC_OUT_F16), kU8 = k1_variant(MDC_OUT_U8);
+    if (out_type == MDC_OUT_F32) return min_ctas <= 2 ? fused_variant_t<2>(tma, vig, pyr) : fused_variant_t<3>(tma, vig, pyr);
+    if (out_type == MDC_OUT_F16) return min_ctas <= 2 ? fused_variant_t<2, kF16>(tma, vig, pyr) : fused_variant_t<3, kF16>(tma, vig, pyr);
+    return min_ctas <= 2 ? fused_variant_t<2, kU8>(tma, vig, pyr) : fused_variant_t<3, kU8>(tma, vig, pyr);
 }
 
-int fused_max_ctas_per_sm(int box_px_max, int stages, bool tma, bool vig, bool pyr, int min_ctas) {
+int fused_max_ctas_per_sm(int box_px_max, int stages, bool tma, bool vig, bool pyr, int min_ctas, int out_type) {
     int n = 0;
     const int smem = static_cast<int>(fused_smem_bytes(box_px_max, stages));
-    FusedKernelFn fn = fused_variant(tma, vig, pyr, min_ctas);
+    FusedKernelFn fn = fused_variant(tma, vig, pyr, min_ctas, out_type);
     // the opt-in limit must be raised before the occupancy query, or it reports 0 for > 48 KB
     if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) return 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn, tma ? kConsumers + 32 : kConsumers, smem) != cudaSuccess) return 0;
     return n;
 }
 
-cudaError_t launch_fused(const FusedParams& p, const TmaMaps* maps, int grid, int min_ctas, cudaStream_t stream) {
+cudaError_t launch_fused(const FusedParams& p, const TmaMaps* maps, int grid, int min_ctas, int out_type, cudaStream_t stream) {
     const bool tma = maps != nullptr;
     const size_t smem = fused_smem_bytes(p.box_px_max, tma ? p.tma_stages : kLdgStages);
-    FusedKernelFn fn = fused_variant(tma, p.use_vig != 0, p.levels > 1, min_ctas);
+    FusedKernelFn fn = fused_variant(tma, p.use_vig != 0, p.levels > 1, min_ctas, out_type);
     cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
     if (e != cudaSuccess) return e;
     if (p.carveout > 0 && (e = cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, p.carveout)) != cudaSuccess) return e;
@@ -580,9 +628,13 @@ __device__ __forceinline__ void tld4_u8(unsigned long long tex, float u, float v
     asm volatile("tld4.r.2d.v4.u32.f32 {%0, %1, %2, %3}, [%4, {%5, %6}];" : "=r"(x), "=r"(y), "=r"(z), "=r"(w) : "l"(tex), "f"(u), "f"(v));
 }
 
+// kStudy: floor-study bits | output type << kOutShift, as for the staged kernel
 template <bool kVig, bool kPyr, int kMinCtas, bool kPrefetch, int kStudy>
 __global__ void __launch_bounds__(kTexThreads, kMinCtas)
 fused_tex_kernel(const __grid_constant__ FusedParams p, const __grid_constant__ TexSet texs) {
+    constexpr int kOut = kStudy >> kOutShift;
+    using TOut = typename OutElem<kOut>::T;     // only the stores depend on it
+    constexpr bool kNarrow = kOut != MDC_OUT_F32;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     float* lut = reinterpret_cast<float*>(smem_raw);                    // [256][32] lane-replicated response LUT
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -655,22 +707,29 @@ fused_tex_kernel(const __grid_constant__ FusedParams p, const __grid_constant__ 
                 vi2[h][k] = pack2(vi[2 * h][k], vi[2 * h + 1][k]);
             }
 
-        float* o0 = p.out[0] + static_cast<size_t>(f_begin) * p.lw[0] * p.lh[0] + static_cast<size_t>(oy0) * p.out_w + ox;
+        TOut* o0 = static_cast<TOut*>(p.out[0]) + static_cast<size_t>(f_begin) * p.lw[0] * p.lh[0] + static_cast<size_t>(oy0) * p.out_w + ox;
         const size_t o0_step = static_cast<size_t>(p.lw[0]) * p.lh[0];
         const bool full_strip = inside == 0xfu;
-        float *o1 = nullptr, *o2 = nullptr;
+        TOut *o1 = nullptr, *o2 = nullptr;
+        float* o2f = nullptr;
         uint32_t o1_step = 0, o2_step = 0;
-        bool st1 = false, st2 = false;
+        bool st1 = false, st2 = false, st2f = false;
         if (kPyr) {
             const int X1 = (tx0 >> 1) + (lane >> 1), Y1 = (ty0 >> 1) + 2 * wrow + (lane & 1);   // even lane: upper block, odd lane: lower block
             st1 = X1 < p.lw[1] && Y1 < p.lh[1];
             o1_step = static_cast<uint32_t>(p.lw[1]) * static_cast<uint32_t>(p.lh[1]);
-            o1 = p.out[1] + static_cast<size_t>(f_begin) * o1_step + static_cast<size_t>(Y1) * p.lw[1] + X1;
+            o1 = static_cast<TOut*>(p.out[1]) + static_cast<size_t>(f_begin) * o1_step + static_cast<size_t>(Y1) * p.lw[1] + X1;
             if (p.levels > 2) {
                 const int X2 = (tx0 >> 2) + (lane >> 2), Y2 = (ty0 >> 2) + wrow;
                 st2 = (lane & 3) == 0 && X2 < p.lw[2] && Y2 < p.lh[2];
                 o2_step = static_cast<uint32_t>(p.lw[2]) * static_cast<uint32_t>(p.lh[2]);
-                o2 = p.out[2] + static_cast<size_t>(f_begin) * o2_step + static_cast<size_t>(Y2) * p.lw[2] + X2;
+                o2 = static_cast<TOut*>(p.out[2]) + static_cast<size_t>(f_begin) * o2_step + static_cast<size_t>(Y2) * p.lw[2] + X2;
+                if constexpr (kNarrow) {
+                    if (p.level2_f32) {
+                        o2f = p.level2_f32 + static_cast<size_t>(f_begin) * o2_step + static_cast<size_t>(Y2) * p.lw[2] + X2;
+                        st2f = st2;
+                    }
+                }
             }
         }
         uint32_t study_acc = 0;
@@ -757,21 +816,38 @@ fused_tex_kernel(const __grid_constant__ FusedParams p, const __grid_constant__ 
                     const float l2 = __fmul_rn(0.25f, __fadd_rn(__fadd_rn(__fadd_rn(l1, b2), c2), d2));   // lanes = 0 mod 4
                     if (st2) stg_cs(o2, l2);
                     o2 += o2_step;
+                    if constexpr (kNarrow) {
+                        if (st2f) stg_cs(o2f, l2);
+                        o2f += o2_step;
+                    }
                 }
             }
         }
-        if (!(kStudy & kStudyStores) && study_acc == 0x9e3779b9u && (inside & 1u)) stg_cs(p.out[0], 0.0f);   // keeps the folded pixels alive
+        if (!(kStudy & kStudyStores) && study_acc == 0x9e3779b9u && (inside & 1u)) stg_cs(static_cast<TOut*>(p.out[0]), 0.0f);   // keeps the folded pixels alive
         }
     }
 }
 
 typedef void (*FusedTexFn)(const FusedParams, const TexSet);
-template <int kMinCtas, bool kPrefetch>
+template <int kMinCtas, bool kPrefetch, int kOut>
 static FusedTexFn fused_tex_variant_t(bool vig, bool pyr) {
-    if (vig) return pyr ? fused_tex_kernel<true, true, kMinCtas, kPrefetch, kStudyAll> : fused_tex_kernel<true, false, kMinCtas, kPrefetch, kStudyAll>;
-    return pyr ? fused_tex_kernel<false, true, kMinCtas, kPrefetch, kStudyAll> : fused_tex_kernel<false, false, kMinCtas, kPrefetch, kStudyAll>;
+    constexpr int V = k1_variant(kOut);
+    if (vig) return pyr ? fused_tex_kernel<true, true, kMinCtas, kPrefetch, V> : fused_tex_kernel<true, false, kMinCtas, kPrefetch, V>;
+    return pyr ? fused_tex_kernel<false, true, kMinCtas, kPrefetch, V> : fused_tex_kernel<false, false, kMinCtas, kPrefetch, V>;
 }
-static FusedTexFn fused_tex_variant(bool vig, bool pyr, int min_ctas, bool prefetch, int study) {
+template <int kOut>
+static FusedTexFn fused_tex_variant_o(bool vig, bool pyr, int min_ctas, bool prefetch) {
+    if (prefetch) {
+        if (min_ctas <= 2) return fused_tex_variant_t<2, true, kOut>(vig, pyr);
+        return min_ctas == 3 ? fused_tex_variant_t<3, true, kOut>(vig, pyr) : fused_tex_variant_t<4, true, kOut>(vig, pyr);
+    }
+    if (min_ctas <= 2) return fused_tex_variant_t<2, false, kOut>(vig, pyr);
+    return min_ctas == 3 ? fused_tex_variant_t<3, false, kOut>(vig, pyr) : fused_tex_variant_t<4, false, kOut>(vig, pyr);
+}
+// study: floor-study variants (fp32 only); out_type: MDC_OUT_*
+static FusedTexFn fused_tex_variant(bool vig, bool pyr, int min_ctas, bool prefetch, int study, int out_type) {
+    if (out_type == MDC_OUT_F16) return fused_tex_variant_o<MDC_OUT_F16>(vig, pyr, min_ctas, prefetch);
+    if (out_type == MDC_OUT_U8) return fused_tex_variant_o<MDC_OUT_U8>(vig, pyr, min_ctas, prefetch);
     if (study != kStudyAll && vig && !pyr) {      // floor study: <vignette, no pyramid, 3 CTAs/SM, no prefetch> with parts disabled
         switch (study & kStudyAll) {
             case 0: return fused_tex_kernel<true, false, 3, false, 0>;
@@ -784,26 +860,22 @@ static FusedTexFn fused_tex_variant(bool vig, bool pyr, int min_ctas, bool prefe
             default: break;
         }
     }
-    if (prefetch) {
-        if (min_ctas <= 2) return fused_tex_variant_t<2, true>(vig, pyr);
-        return min_ctas == 3 ? fused_tex_variant_t<3, true>(vig, pyr) : fused_tex_variant_t<4, true>(vig, pyr);
-    }
-    if (min_ctas <= 2) return fused_tex_variant_t<2, false>(vig, pyr);
-    return min_ctas == 3 ? fused_tex_variant_t<3, false>(vig, pyr) : fused_tex_variant_t<4, false>(vig, pyr);
+    return fused_tex_variant_o<MDC_OUT_F32>(vig, pyr, min_ctas, prefetch);
 }
 constexpr int kTexSmemBytes = 256 * 32 * 4;
 
 int fused_tex_max_ctas_per_sm(bool vig, bool pyr, int min_ctas, bool prefetch) {
     int n = 0;
-    FusedTexFn fn = fused_tex_variant(vig, pyr, min_ctas, prefetch, kStudyAll);
+    FusedTexFn fn = fused_tex_variant(vig, pyr, min_ctas, prefetch, kStudyAll, MDC_OUT_F32);
     if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kTexSmemBytes) != cudaSuccess) return 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn, kTexThreads, kTexSmemBytes) != cudaSuccess) return 0;
     return n;
 }
 
-cudaError_t launch_fused_tex(const FusedParams& p, const TexSet& texs, int n_chunks, int min_ctas, bool prefetch, int study, cudaStream_t stream) {
+cudaError_t launch_fused_tex(const FusedParams& p, const TexSet& texs, int n_chunks, int min_ctas, bool prefetch, int study, int out_type,
+                             cudaStream_t stream) {
     if (n_chunks < 1 || n_chunks > kMaxTex || p.tiles_per_cta < 1) return cudaErrorInvalidValue;
-    FusedTexFn fn = fused_tex_variant(p.use_vig != 0, p.levels > 1, min_ctas, prefetch, study);
+    FusedTexFn fn = fused_tex_variant(p.use_vig != 0, p.levels > 1, min_ctas, prefetch, study, out_type);
     cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kTexSmemBytes);
     if (e != cudaSuccess) return e;
     if (p.carveout > 0 && (e = cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, p.carveout)) != cudaSuccess) return e;
@@ -829,11 +901,15 @@ cudaError_t launch_count_mismatch(const void* a, const void* b, size_t n_words, 
 }
 
 // =====================================================================================
-// K1a: unMapImage alone (streaming; 1 B in, 4 B out, 4 B vignette per pixel)
+// K1a: unMapImage alone (streaming; 1 B in, 4 B out, 4 B vignette per pixel).  T = output element; a narrow T converts at the
+// store and, where a K2 pass reads this level, also writes the fp32 pixels to out_f32 (a trailing parameter, so that the float
+// instantiation keeps the parameter offsets and the code of the fp32-only kernel).
 // =====================================================================================
-__global__ void __launch_bounds__(256) unmap_kernel(const uint8_t* __restrict__ in, float* __restrict__ out, size_t n,
+template <typename T>
+__global__ void __launch_bounds__(256) unmap_kernel(const uint8_t* __restrict__ in, T* __restrict__ out, size_t n,
                                                     int n_frames, const float* __restrict__ ginv,
-                                                    const float* __restrict__ vinv, unsigned kill) {
+                                                    const float* __restrict__ vinv, unsigned kill, float* __restrict__ out_f32) {
+    constexpr bool kNarrow = !std::is_same<T, float>::value;
     __shared__ float lut[256];
     {
         float v = ginv ? ginv[threadIdx.x] : static_cast<float>(threadIdx.x);
@@ -842,8 +918,9 @@ __global__ void __launch_bounds__(256) unmap_kernel(const uint8_t* __restrict__ 
     }
     __syncthreads();
     const size_t total = n * static_cast<size_t>(n_frames);
-    const bool vec = ((n & 3) == 0) && ((reinterpret_cast<uintptr_t>(in) & 3) == 0) && ((reinterpret_cast<uintptr_t>(out) & 15) == 0) &&
-                     (!vinv || (reinterpret_cast<uintptr_t>(vinv) & 15) == 0);
+    bool vec = ((n & 3) == 0) && ((reinterpret_cast<uintptr_t>(in) & 3) == 0) && ((reinterpret_cast<uintptr_t>(out) & (4 * sizeof(T) - 1)) == 0) &&
+               (!vinv || (reinterpret_cast<uintptr_t>(vinv) & 15) == 0);
+    if constexpr (kNarrow) vec = vec && (reinterpret_cast<uintptr_t>(out_f32) & 15) == 0;
     const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
     if (vec) {
         const size_t words = total >> 2, nw = n >> 2;
@@ -854,25 +931,34 @@ __global__ void __launch_bounds__(256) unmap_kernel(const uint8_t* __restrict__ 
                 const float4 m = __ldg(reinterpret_cast<const float4*>(vinv) + (i % nw));
                 o.x = __fmul_rn(o.x, m.x); o.y = __fmul_rn(o.y, m.y); o.z = __fmul_rn(o.z, m.z); o.w = __fmul_rn(o.w, m.w);
             }
-            reinterpret_cast<float4*>(out)[i] = o;
+            if constexpr (kNarrow) {
+                put4(out + 4 * i, o);
+                if (out_f32) reinterpret_cast<float4*>(out_f32)[i] = o;
+            } else {
+                reinterpret_cast<float4*>(out)[i] = o;
+            }
         }
     } else {
         for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += stride) {
             float o = lut[in[i]];
             if (vinv) o = __fmul_rn(o, __ldg(vinv + (i % n)));
-            out[i] = o;
+            put(out + i, o);
+            if constexpr (kNarrow) if (out_f32) out_f32[i] = o;
         }
     }
 }
 
-cudaError_t launch_unmap(const uint8_t* in, float* out, size_t n, int n_frames, const float* ginv, const float* vinv,
-                         unsigned kill, cudaStream_t stream) {
+cudaError_t launch_unmap(const uint8_t* in, void* out, int out_type, float* out_f32, size_t n, int n_frames, const float* ginv,
+                         const float* vinv, unsigned kill, cudaStream_t stream) {
     const size_t total = n * static_cast<size_t>(n_frames);
     if (total == 0) return cudaSuccess;
     size_t blocks = (total / 4 + 255) / 256;
     blocks = std::min(blocks, grid_cap(16));
     if (blocks < 1) blocks = 1;
-    unmap_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(in, out, n, n_frames, ginv, vinv, kill);
+    const unsigned g = static_cast<unsigned>(blocks);
+    if (out_type == MDC_OUT_F16) unmap_kernel<<<g, 256, 0, stream>>>(in, static_cast<__half*>(out), n, n_frames, ginv, vinv, kill, out_f32);
+    else if (out_type == MDC_OUT_U8) unmap_kernel<<<g, 256, 0, stream>>>(in, static_cast<uint8_t*>(out), n, n_frames, ginv, vinv, kill, out_f32);
+    else unmap_kernel<<<g, 256, 0, stream>>>(in, static_cast<float*>(out), n, n_frames, ginv, vinv, kill, nullptr);
     return cudaGetLastError();
 }
 
@@ -916,10 +1002,13 @@ cudaError_t launch_undistort_f32(const float* in, float* out, int in_w, int n_in
 }
 
 // =====================================================================================
-// K2: stand-alone pyramid level (used for levels beyond the fused epilogue and for API parity)
+// K2: stand-alone pyramid level (used for levels beyond the fused epilogue and for API parity).  The source is always fp32; T is
+// the destination element, and a narrow T also writes the fp32 level to dst_f32 when a later pass reads it (trailing parameter,
+// as for unmap_kernel).
 // =====================================================================================
-__global__ void __launch_bounds__(256) pyr_down_kernel(const float* __restrict__ src, int sw, int sh, float* __restrict__ dst,
-                                                       int n_frames) {
+template <typename T>
+__global__ void __launch_bounds__(256) pyr_down_kernel(const float* __restrict__ src, int sw, int sh, T* __restrict__ dst,
+                                                       int n_frames, float* __restrict__ dst_f32) {
     const int dw = sw >> 1, dh = sh >> 1;
     const size_t per = static_cast<size_t>(dw) * dh, total = per * n_frames;
     const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
@@ -927,15 +1016,19 @@ __global__ void __launch_bounds__(256) pyr_down_kernel(const float* __restrict__
         const size_t f = i / per, r = i - f * per;
         const int y = static_cast<int>(r / dw), x = static_cast<int>(r - static_cast<size_t>(y) * dw);
         const float* s = src + f * static_cast<size_t>(sw) * sh + static_cast<size_t>(2 * y) * sw + 2 * x;
-        dst[i] = __fmul_rn(0.25f, __fadd_rn(__fadd_rn(__fadd_rn(__ldg(s), __ldg(s + 1)), __ldg(s + sw)), __ldg(s + sw + 1)));
+        const float v = __fmul_rn(0.25f, __fadd_rn(__fadd_rn(__fadd_rn(__ldg(s), __ldg(s + 1)), __ldg(s + sw)), __ldg(s + sw + 1)));
+        put(dst + i, v);
+        if constexpr (!std::is_same<T, float>::value) if (dst_f32) dst_f32[i] = v;
     }
 }
 
 // Two levels in one pass (used for levels 3+4 behind the fused kernel): each thread owns one 2x2 block of the first
 // destination level — i.e. a 4x4 block of the source — writes those up to 4 pixels and, if complete, the pixel of the
-// second destination level.  Same arithmetic as two pyr_down_kernel passes (the intermediate values are identical).
-__global__ void __launch_bounds__(256) pyr_down2_kernel(const float* __restrict__ src, int sw, int sh, float* __restrict__ d1,
-                                                        float* __restrict__ d2, int n_frames) {
+// second destination level.  Same arithmetic as two pyr_down_kernel passes (the intermediate values are identical): the first
+// level's pixels stay fp32 in registers whatever T is, and a narrow T writes the second level's fp32 pixels to d2_f32 as well.
+template <typename T>
+__global__ void __launch_bounds__(256) pyr_down2_kernel(const float* __restrict__ src, int sw, int sh, T* __restrict__ d1,
+                                                        T* __restrict__ d2, int n_frames, float* __restrict__ d2_f32) {
     const int w1 = sw >> 1, h1 = sh >> 1, w2 = w1 >> 1, h2 = h1 >> 1;
     const int bw = (w1 + 1) >> 1, bh = (h1 + 1) >> 1;
     const size_t per = static_cast<size_t>(bw) * bh, total = per * n_frames;
@@ -953,30 +1046,43 @@ __global__ void __launch_bounds__(256) pyr_down2_kernel(const float* __restrict_
                 if (x < w1 && y < h1) {
                     const float* q = s + static_cast<size_t>(2 * y) * sw + 2 * x;
                     v[dy][dx] = __fmul_rn(0.25f, __fadd_rn(__fadd_rn(__fadd_rn(__ldg(q), __ldg(q + 1)), __ldg(q + sw)), __ldg(q + sw + 1)));
-                    d1[f * static_cast<size_t>(w1) * h1 + static_cast<size_t>(y) * w1 + x] = v[dy][dx];
+                    put(d1 + (f * static_cast<size_t>(w1) * h1 + static_cast<size_t>(y) * w1 + x), v[dy][dx]);
                 }
             }
-        if (bx < w2 && by < h2)
-            d2[f * static_cast<size_t>(w2) * h2 + static_cast<size_t>(by) * w2 + bx] =
-                __fmul_rn(0.25f, __fadd_rn(__fadd_rn(__fadd_rn(v[0][0], v[0][1]), v[1][0]), v[1][1]));
+        if (bx < w2 && by < h2) {
+            const size_t o = f * static_cast<size_t>(w2) * h2 + static_cast<size_t>(by) * w2 + bx;
+            const float v2 = __fmul_rn(0.25f, __fadd_rn(__fadd_rn(__fadd_rn(v[0][0], v[0][1]), v[1][0]), v[1][1]));
+            put(d2 + o, v2);
+            if constexpr (!std::is_same<T, float>::value) if (d2_f32) d2_f32[o] = v2;
+        }
     }
 }
 
-cudaError_t launch_pyr_down2(const float* src, int sw, int sh, float* d1, float* d2, int n_frames, cudaStream_t stream) {
+cudaError_t launch_pyr_down2(const float* src, int sw, int sh, void* d1, void* d2, int out_type, float* d2_f32, int n_frames,
+                             cudaStream_t stream) {
     const size_t total = static_cast<size_t>(((sw >> 1) + 1) >> 1) * (((sh >> 1) + 1) >> 1) * n_frames;
     if (total == 0) return cudaSuccess;
     size_t blocks = (total + 255) / 256;
     blocks = std::min(blocks, grid_cap(16));
-    pyr_down2_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(src, sw, sh, d1, d2, n_frames);
+    const unsigned g = static_cast<unsigned>(blocks);
+    if (out_type == MDC_OUT_F16)
+        pyr_down2_kernel<<<g, 256, 0, stream>>>(src, sw, sh, static_cast<__half*>(d1), static_cast<__half*>(d2), n_frames, d2_f32);
+    else if (out_type == MDC_OUT_U8)
+        pyr_down2_kernel<<<g, 256, 0, stream>>>(src, sw, sh, static_cast<uint8_t*>(d1), static_cast<uint8_t*>(d2), n_frames, d2_f32);
+    else
+        pyr_down2_kernel<<<g, 256, 0, stream>>>(src, sw, sh, static_cast<float*>(d1), static_cast<float*>(d2), n_frames, nullptr);
     return cudaGetLastError();
 }
 
-cudaError_t launch_pyr_down(const float* src, int sw, int sh, float* dst, int n_frames, cudaStream_t stream) {
+cudaError_t launch_pyr_down(const float* src, int sw, int sh, void* dst, int out_type, float* dst_f32, int n_frames, cudaStream_t stream) {
     const size_t total = static_cast<size_t>(sw >> 1) * (sh >> 1) * n_frames;
     if (total == 0) return cudaSuccess;
     size_t blocks = (total + 255) / 256;
     blocks = std::min(blocks, grid_cap(16));
-    pyr_down_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(src, sw, sh, dst, n_frames);
+    const unsigned g = static_cast<unsigned>(blocks);
+    if (out_type == MDC_OUT_F16) pyr_down_kernel<<<g, 256, 0, stream>>>(src, sw, sh, static_cast<__half*>(dst), n_frames, dst_f32);
+    else if (out_type == MDC_OUT_U8) pyr_down_kernel<<<g, 256, 0, stream>>>(src, sw, sh, static_cast<uint8_t*>(dst), n_frames, dst_f32);
+    else pyr_down_kernel<<<g, 256, 0, stream>>>(src, sw, sh, static_cast<float*>(dst), n_frames, nullptr);
     return cudaGetLastError();
 }
 

@@ -3,6 +3,7 @@
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
+#include <stddef.h>
 #include <stdint.h>
 
 #include "mdc_b200.h"
@@ -56,7 +57,9 @@ struct FusedParams {
     const TileDesc* tiles;       // [tiles_x*tiles_y]
     int* work_counter;           // zeroed before the launch; item = gridDim.x + atomicAdd(work_counter, 1)
     int tiles_x, n_tiles;
-    float* out[MDC_MAX_PYR_LEVELS];
+    void* out[kInKernelLevels];  // levels 0..levels-1, elements of the launch's output type (MDC_OUT_*)
+    float* level2_f32;           // narrow output types only: fp32 copy of level 2 for the K2 chain behind K1, or nullptr
+    void* unused_[MDC_MAX_PYR_LEVELS - kInKernelLevels - 1];   // room for eight level pointers: the parameter offsets (and the fp32 code) stay
     int lw[MDC_MAX_PYR_LEVELS], lh[MDC_MAX_PYR_LEVELS];
     int levels;                  // 1..kInKernelLevels (levels written by K1 itself)
     unsigned lut_gamma, use_vig, kill;   // sanitised unMapImage flags
@@ -66,27 +69,36 @@ struct FusedParams {
     int tiles_per_cta;           // texture-gather loader: consecutive tiles one CTA works through (grid.x = ceil(n_tiles / tiles_per_cta))
     int carveout;                // host side only: preferred shared-memory carve-out in percent for this launch, 0 = the driver's choice
 };
+static_assert(sizeof(FusedParams) == 256 && offsetof(FusedParams, lw) == 152, "FusedParams layout: the kernels' parameter offsets");
 
 // Floor-study switches (scripts/k1_study.py): which of the three shared-memory/LSU consumers of the frame loop run.
 // kStudyAll is the product; the others replace the disabled part by one or two ALU instructions so that the rest can be timed alone.
 enum StudyBits : int { kStudyTaps = 1, kStudyLut = 2, kStudyStores = 4, kStudyAll = 7 };
+// The K1 kernels' variant parameter: the study bits, and above them the output type (MDC_OUT_*) the levels are stored as.
+constexpr int kOutShift = 8;
+constexpr int k1_variant(int out_type, int study = kStudyAll) { return study | out_type << kOutShift; }
 
 size_t fused_smem_bytes(int box_px_max, int stages);
 int fused_tma_stages(int box_px_max, int ctas_per_sm);
-cudaError_t launch_fused(const FusedParams& p, const TmaMaps* maps, int grid, int min_ctas, cudaStream_t stream);  // maps == nullptr: LDG loader
-int fused_max_ctas_per_sm(int box_px_max, int stages, bool tma, bool vig, bool pyr, int min_ctas);
+// out_type (MDC_OUT_*): element type of p.out[]; every type computes the fp32 levels and converts them at the store
+cudaError_t launch_fused(const FusedParams& p, const TmaMaps* maps, int grid, int min_ctas, int out_type, cudaStream_t stream);  // maps == nullptr: LDG loader
+int fused_max_ctas_per_sm(int box_px_max, int stages, bool tma, bool vig, bool pyr, int min_ctas, int out_type);
 cudaError_t launch_fused_study(const FusedParams& p, const TmaMaps* maps, int grid, int study, cudaStream_t stream);   // <tma, vig, no pyramid, 3 CTAs/SM> only
 // texture-gather loader (taps through the TEX pipe, LUT + stores through the LSU pipe)
-cudaError_t launch_fused_tex(const FusedParams& p, const TexSet& texs, int n_chunks, int min_ctas, bool prefetch, int study, cudaStream_t stream);
+cudaError_t launch_fused_tex(const FusedParams& p, const TexSet& texs, int n_chunks, int min_ctas, bool prefetch, int study, int out_type,
+                             cudaStream_t stream);
 int fused_tex_max_ctas_per_sm(bool vig, bool pyr, int min_ctas, bool prefetch);
 cudaError_t launch_count_mismatch(const void* a, const void* b, size_t n_words, unsigned long long* out, cudaStream_t stream);
 
-cudaError_t launch_unmap(const uint8_t* in, float* out, size_t n, int n_frames, const float* ginv, const float* vinv,
-                         unsigned kill, cudaStream_t stream);
+// out: elements of out_type; out_f32 (narrow types only, may be nullptr): the same pixels as fp32, for a K2 pass that reads them
+cudaError_t launch_unmap(const uint8_t* in, void* out, int out_type, float* out_f32, size_t n, int n_frames, const float* ginv,
+                         const float* vinv, unsigned kill, cudaStream_t stream);
 cudaError_t launch_undistort_f32(const float* in, float* out, int in_w, int n_in, int n_out, int n_frames,
                                  const float* remap_x, const float* remap_y, cudaStream_t stream);
-cudaError_t launch_pyr_down(const float* src, int sw, int sh, float* dst, int n_frames, cudaStream_t stream);
-cudaError_t launch_pyr_down2(const float* src, int sw, int sh, float* d1, float* d2, int n_frames, cudaStream_t stream);
+// K2 reads fp32 levels and writes out_type; dst_f32 / d2_f32 (narrow types only, may be nullptr) get the fp32 result as well
+cudaError_t launch_pyr_down(const float* src, int sw, int sh, void* dst, int out_type, float* dst_f32, int n_frames, cudaStream_t stream);
+cudaError_t launch_pyr_down2(const float* src, int sw, int sh, void* d1, void* d2, int out_type, float* d2_f32, int n_frames,
+                             cudaStream_t stream);
 // per-calibration constants of distortCoordinates (same ten floats as mdc_distort_constants on the host side)
 struct DistortConstants { float ocx, ocy, ofx, ofy, d2t, omega, fx, fy, cx, cy; };
 cudaError_t launch_fov_distort(float* xs, float* ys, size_t n, const DistortConstants& k, cudaStream_t stream);

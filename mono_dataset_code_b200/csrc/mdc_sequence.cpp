@@ -302,8 +302,21 @@ int mdc_seq_default_threads() {
 }
 
 // getImage(id, ...) for ids [first, first+count): decode ahead on `threads` host threads, prepare on the GPU chunk by chunk.
+namespace {
+int prepare_host_f32(mdc_ctx* c, const uint8_t* frames, int n_frames, unsigned flags, int, void* const* out_levels, int levels) {
+    return mdc_prepare_batch_host(c, frames, n_frames, flags, reinterpret_cast<float* const*>(out_levels), levels);
+}
+}  // namespace
+
 extern "C" int mdc_seq_prepare(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned flags, float* const* h_out_levels, int levels,
                                int threads) {
+    return mdc_seq_prepare_feed(c, s, first, count, flags, MDC_OUT_F32, reinterpret_cast<void* const*>(h_out_levels), levels, threads,
+                                prepare_host_f32);
+}
+
+// mdc_seq_prepare(_ex): out_type is already checked (mdc_seq_prepare_ex, mdc_capi.cu); `prepare` takes each decoded chunk.
+int mdc_seq_prepare_feed(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned flags, int out_type, void* const* h_out_levels,
+                         int levels, int threads, mdc_host_prepare_fn prepare) {
     // Everything that does not depend on the context is checked first, and all of it before any staging or thread work.  The range
     // test is written so that it cannot overflow (first + count can).
     if (!s || !h_out_levels) { mdc_set_error("mdc_seq_prepare: bad argument"); return MDC_ERR_INVALID_ARG; }
@@ -419,9 +432,11 @@ extern "C" int mdc_seq_prepare(mdc_ctx* c, const mdc_seq* s, int first, int coun
             break;
         }
         const int f0 = k * chunk, n = std::min(chunk, count - f0);
-        std::vector<float*> outs(static_cast<size_t>(levels));
-        for (int l = 0; l < levels; ++l) outs[static_cast<size_t>(l)] = h_out_levels[l] ? h_out_levels[l] + static_cast<size_t>(f0) * level_px[static_cast<size_t>(l)] : nullptr;
-        rc = mdc_prepare_batch_host(c, static_cast<const uint8_t*>(stage[k & 1]), n, flags, outs.data(), levels);      // returns after the D2H copy
+        std::vector<void*> outs(static_cast<size_t>(levels));
+        const size_t esize = mdc_out_elem_size(out_type);
+        for (int l = 0; l < levels; ++l)
+            outs[static_cast<size_t>(l)] = h_out_levels[l] ? static_cast<uint8_t*>(h_out_levels[l]) + static_cast<size_t>(f0) * level_px[static_cast<size_t>(l)] * esize : nullptr;
+        rc = prepare(c, static_cast<const uint8_t*>(stage[k & 1]), n, flags, out_type, outs.data(), levels);      // returns after the D2H copy
         std::lock_guard<std::mutex> lk(mu);
         released = k + 2;             // stage[k & 1] is free again: chunk k+2 may be decoded into it
         cv.notify_all();
