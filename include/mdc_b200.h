@@ -287,6 +287,18 @@ int mdc_seq_read_gray8_device(mdc_ctx* c, const mdc_seq* s, const int* ids, int 
  * failed frames untouched.  Uses the context's device; `stream` as for mdc_prepare_batch; returns when the frames are decoded. */
 int mdc_jpeg_decode_device(mdc_ctx* c, const uint8_t* const* files, const size_t* sizes, int n, int w, int h, uint8_t* d_out,
                            size_t row_pitch, int* status_host, mdc_stream stream);
+/* Bytes the file of a w x h frame can take at any quality 1..100 (header, worst-case code of every block, stuffing, EOI); 0 unless
+ * 1 <= w, h <= 65535. */
+size_t mdc_jpeg_encode_bound(int w, int h);
+/* cv::imwrite(".jpg") of a single-channel 8-bit image with quality `quality` (OpenCV's default: 95): d_frames [n][h][row_pitch]
+ * u8 on the device -> frame k's complete JFIF file at d_out + k*out_stride (DEVICE), its length in sizes_host[k].  The bytes are
+ * libjpeg's baseline defaults for one component (standard Huffman tables, accurate integer DCT, no restart markers), the same on
+ * every run.  Padding bytes of the input rows are never read; bytes of d_out past a frame's size are unspecified.
+ * MDC_ERR_INVALID_ARG before any kernel runs for a NULL c, n < 0, quality outside 1..100, w or h outside 1..65535, row_pitch < w,
+ * out_stride < mdc_jpeg_encode_bound(w, h), or a NULL d_frames, d_out or sizes_host with n > 0; n = 0 is a no-op.  Uses the context's
+ * device; `stream` as for mdc_prepare_batch; returns when the files are on the device. */
+int mdc_jpeg_encode_device(mdc_ctx* c, const uint8_t* d_frames, size_t row_pitch, int n, int w, int h, int quality,
+                           uint8_t* d_out, size_t out_stride, size_t* sizes_host, mdc_stream stream);
 
 /* =====================================================================================
  * vignetteCalib optimiser, main_vignetteCalib.cpp:395-585 (SURVEY.md §8f N4).  Everything is device-resident, contiguous:

@@ -52,6 +52,9 @@ SIGNATURES = {
     "mdc_seq_read_gray8_device": (C.c_int, [_vp, _vp, _vp, C.c_int, C.c_int, C.c_int, _vp, C.c_size_t, _vp, _vp, C.c_int, _vp]),
     "mdc_jpeg_decode_device": (C.c_int, [_vp, C.POINTER(_vp), C.POINTER(C.c_size_t), C.c_int, C.c_int, C.c_int, _vp, C.c_size_t,
                                          C.POINTER(C.c_int), _vp]),
+    "mdc_jpeg_encode_bound": (C.c_size_t, [C.c_int, C.c_int]),
+    "mdc_jpeg_encode_device": (C.c_int, [_vp, _vp, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, _vp, C.c_size_t,
+                                         C.POINTER(C.c_size_t), _vp]),
     "mdc_vc_plane_step": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _vp, _vp, C.c_double, C.c_int, C.POINTER(C.c_double)]),
     "mdc_vc_vignette_step": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _vp, _vp, C.c_double, C.c_int, C.POINTER(C.c_double)]),
     "mdc_vc_smooth": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, _vp]),

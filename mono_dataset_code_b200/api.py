@@ -720,6 +720,36 @@ def jpeg_decode_device(blobs, w: int, h: int, ctx: "Context | None" = None, devi
     return out, np.array(status[:n], dtype=np.int32)
 
 
+def jpeg_encode_bound(w: int, h: int) -> int:
+    """Bytes the JPEG file of a w x h frame can take at any quality (mdc_jpeg_encode_bound)."""
+    return int(lib.mdc_jpeg_encode_bound(w, h))
+
+
+def jpeg_encode_device(frames, quality: int = 95, ctx: "Context | None" = None, device: int = 0, row_pitch: int | None = None) -> list:
+    """cv2.imencode('.jpg', frame, [cv2.IMWRITE_JPEG_QUALITY, quality]) of every frame, encoded on the GPU (mdc_jpeg_encode_device):
+    frames is a uint8 CUDA tensor [n, h, w] whose rows may be padded, e.g. a [:, :, :w] slice of a [n, h, pitch] buffer; the padding is
+    never read.  row_pitch defaults to the tensor's row stride.  Runs on torch's current stream; returns the n files as bytes."""
+    import torch
+    if frames.dtype != torch.uint8 or not frames.is_cuda or frames.dim() != 3 or (frames.shape[0] and frames.shape[2] and frames.stride(2) != 1):
+        raise ValueError("jpeg_encode_device: frames must be a uint8 CUDA tensor [n, h, w] with unit stride along w")
+    n, h, w = frames.shape
+    pitch = row_pitch if row_pitch is not None else frames.stride(1)
+    if n > 1 and frames.stride(0) != h * pitch:
+        raise ValueError("jpeg_encode_device: frames must be h * row_pitch bytes apart")
+    if ctx is None:
+        ctx = Context(None, None, frames.device.index if frames.device.index is not None else device)
+    stride = jpeg_encode_bound(w, h)
+    out = torch.empty((n, max(stride, 1)), dtype=torch.uint8, device=frames.device)
+    sizes = (C.c_size_t * max(n, 1))()
+    check(lib.mdc_jpeg_encode_device(ctx._h, C.c_void_p(frames.data_ptr()), pitch, n, w, h, quality, C.c_void_p(out.data_ptr()), stride,
+                                     sizes, Context._stream(out)), "mdc_jpeg_encode_device")
+    if n == 0:
+        return []
+    packed = torch.cat([out[k, :sizes[k]] for k in range(n)]).cpu().numpy().tobytes()      # only the files' bytes cross to the host
+    ends = np.cumsum([sizes[k] for k in range(n)])
+    return [packed[e - sizes[k]:e] for k, e in enumerate(ends)]
+
+
 def atanf_host(x: np.ndarray) -> np.ndarray:
     """The restated glibc atanf (csrc/mdc_atanf.h) evaluated on the host."""
     x = np.ascontiguousarray(x, dtype=np.float32)

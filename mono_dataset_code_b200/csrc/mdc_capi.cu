@@ -1106,6 +1106,12 @@ extern "C" int mdc_atanf_device(const float* d_in, float* d_out, size_t n, int d
 int mdc_ctx_device_ordinal(const mdc_ctx* c) { return c->device; }
 void* mdc_ctx_stream_handle(mdc_ctx* c) { return c->stream; }
 void mdc_ctx_add_launches(mdc_ctx* c, int n) { c->launches += n; }
+int mdc_ctx_scratch_pool(mdc_ctx* c, void** pool) {
+    cudaMemPool_t p = nullptr;
+    const int rc = f32_pool(c, &p);
+    *pool = p;
+    return rc;
+}
 void mdc_ctx_geometry(const mdc_ctx* c, int* in_w, int* in_h, int* out_w, int* out_h) { *in_w = c->in_w; *in_h = c->in_h; *out_w = c->out_w; *out_h = c->out_h; }
 
 extern "C" int mdc_estep(mdc_ctx* c, const uint8_t* d_data, int n, int npix, const double* d_t, const double* d_G, double* d_E, mdc_stream stream) {

@@ -61,6 +61,7 @@ void mdc_photo_set_vignette(mdc_photo* p, const void* pixels, int depth);
 int mdc_ctx_device_ordinal(const mdc_ctx* c);
 void* mdc_ctx_stream_handle(mdc_ctx* c);          // the context's own cudaStream_t
 void mdc_ctx_add_launches(mdc_ctx* c, int n);
+int mdc_ctx_scratch_pool(mdc_ctx* c, void** pool);      // the context's cudaMemPool_t for stream-ordered scratch, kept warm between calls
 void mdc_ctx_geometry(const mdc_ctx* c, int* in_w, int* in_h, int* out_w, int* out_h);
 
 // Sequence internals used by the GPU-decoding feed (mdc_jpeg_gpu.cu).
