@@ -42,7 +42,8 @@ def build(force: bool = False, verbose: bool = False) -> str:
     inc = ["-I" + os.path.join(ROOT, "include"), "-I" + CSRC]
     headers = [os.path.join(ROOT, "include", "mdc_b200.h"), os.path.join(CSRC, "mdc_internal.h"),
                os.path.join(CSRC, "mdc_kernels.cuh"), os.path.join(CSRC, "mdc_atanf.h"), os.path.join(CSRC, "mdc_jpeg.h"),
-               os.path.join(CSRC, "mdc_jpeg_entropy.cuh"), os.path.join(CSRC, "mdc_jpeg_encode.cuh"), os.path.abspath(__file__)]
+               os.path.join(CSRC, "mdc_jpeg_entropy.cuh"), os.path.join(CSRC, "mdc_jpeg_encode.cuh"), os.path.join(CSRC, "mdc_feed.h"),
+               os.path.abspath(__file__)]
     obj_dir = os.path.join(PKG, "build")
     os.makedirs(obj_dir, exist_ok=True)
     os.makedirs(LIB_DIR, exist_ok=True)

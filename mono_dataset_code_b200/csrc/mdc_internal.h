@@ -65,10 +65,25 @@ int mdc_ctx_scratch_pool(mdc_ctx* c, void** pool);      // the context's cudaMem
 void mdc_ctx_geometry(const mdc_ctx* c, int* in_w, int* in_h, int* out_w, int* out_h);
 
 // Sequence internals used by the GPU-decoding feed (mdc_jpeg_gpu.cu).
-struct mdc_seq_feed_stage { void* pinned[2] = {nullptr, nullptr}; size_t bytes[2] = {0, 0}; };      // pinned, kept between calls
+struct mdc_seq_feed_stage {      // a feed's two pinned staging slots, kept between calls
+    void* pinned[2] = {nullptr, nullptr};
+    size_t bytes[2] = {0, 0};
+    void free_slot(int b) { mdc_host_free(pinned[b]); pinned[b] = nullptr; bytes[b] = 0; }
+};
 bool mdc_seq_read_file(const mdc_seq* s, int id, std::vector<uint8_t>* file);      // frame id's file bytes (folder file or zip entry)
 std::mutex& mdc_seq_feed_mutex(const mdc_seq* s);                                   // one feed at a time per sequence object
 mdc_seq_feed_stage* mdc_seq_device_stage(const mdc_seq* s);
+// 8-bit pixels of a decoded frame, as mdc_seq_read_gray8 returns them: a 16-bit image keeps its high byte (img.px is taken when 8-bit)
+void mdc_gray_to_u8(mdc_gray_image& img, std::vector<uint8_t>* px);
+// "expected image dimensions <w> x <h>; found <fw> x <fh> (<what>)", BenchmarkDatasetReader.h:194-199
+std::string mdc_dims_message(int w, int h, int fw, int fh, const std::string& what);
+// The argument checks of mdc_seq_prepare(_ex) and mdc_seq_prepare_device(_ex), "<who>: " messages: first those that need no context
+// (sequence and level array, frame range, level count), then the context's input geometry, then a NULL level that has pixels.  On
+// MDC_OK, *in_w x *in_h is the input size and level_px[l] the pixels per frame of level l of getImage's result.
+int mdc_seq_check_prepare(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned flags, void* const* out_levels, int levels,
+                          const char* who, int* in_w, int* in_h, size_t level_px[MDC_MAX_PYR_LEVELS]);
+// The level pointers of the chunk that starts at frame f0 of a call's output (a NULL level stays NULL).
+std::vector<void*> mdc_seq_chunk_levels(void* const* out_levels, int levels, const size_t* level_px, int out_type, int f0);
 // The decode-ahead host feed behind mdc_seq_prepare and mdc_seq_prepare_ex (mdc_sequence.cpp).  Each decoded chunk goes to `prepare`
 // (mdc_prepare_batch_host_ex's signature), so that the sequence reader calls nothing of the GPU side but what its caller hands it.
 typedef int (*mdc_host_prepare_fn)(mdc_ctx* c, const uint8_t* frames, int n_frames, unsigned flags, int out_type, void* const* out_levels,

@@ -6,14 +6,12 @@
 //   J2     inverse DCT: eight threads per 8x8 block (a column each, then a row each), exactly mdcj::idct_block; cropped samples
 //          into a u8 batch [n][h][row_pitch]
 //   errors per frame in a status word (the first failing segment and its kind), never a trap
-// mdc_jpeg_decode_device decodes host buffers.  One device feed (run_device_feed) reads a sequence's frames on host threads and sends
-// them H2D -> J1 -> J2 chunk by chunk: mdc_seq_prepare_device runs K1 on each chunk, mdc_seq_read_gray8_device leaves the raw frames in
-// the caller's rows.
+// mdc_jpeg_decode_device decodes host buffers.  One device feed (run_device_feed) reads a sequence's frames on the decode-ahead pool
+// (mdc_feed.h) and sends them H2D -> J1 -> J2 chunk by chunk: mdc_seq_prepare_device runs K1 on each chunk, mdc_seq_read_gray8_device
+// leaves the raw frames in the caller's rows.
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <atomic>
-#include <condition_variable>
 #include <cstdio>
 #include <cstring>
 #include <exception>
@@ -22,9 +20,9 @@
 #include <memory>
 #include <mutex>
 #include <string>
-#include <thread>
 #include <vector>
 
+#include "mdc_feed.h"
 #include "mdc_internal.h"
 #include "mdc_jpeg.h"
 
@@ -190,11 +188,14 @@ struct HostBatch {
     }
 };
 
-const char* kind_message(uint32_t st) {
+// A decoded frame's message: the kind of the first interval J1 failed in (status word st), else the host's "missing restart
+// marker" verdict (`incomplete`, "" if the scan is complete), as the host decoder reports them.  "" for a frame that decoded.
+std::string frame_message(uint32_t st, const std::string& name, const std::string& incomplete) {
+    if (st == kStatusOk) return incomplete;
     switch (st & 3) {
-        case mdcj::kBlockBadDc: return "corrupt JPEG data (DC)";
-        case mdcj::kBlockBadAc: return "corrupt JPEG data (AC)";
-        default: return "corrupt JPEG data (run past the block)";
+        case mdcj::kBlockBadDc: return name + ": corrupt JPEG data (DC)";
+        case mdcj::kBlockBadAc: return name + ": corrupt JPEG data (AC)";
+        default: return name + ": corrupt JPEG data (run past the block)";
     }
 }
 
@@ -282,9 +283,7 @@ extern "C" int mdc_jpeg_decode_device(mdc_ctx* c, const uint8_t* const* files, c
                 continue;
             }
             if (hdr.width != w || hdr.height != h) {
-                char m[256];
-                snprintf(m, sizeof m, "expected image dimensions %d x %d; found %d x %d (%s)", w, h, hdr.width, hdr.height, name.c_str());
-                msg[static_cast<size_t>(i)] = m;
+                msg[static_cast<size_t>(i)] = mdc_dims_message(w, h, hdr.width, hdr.height, name);
                 b.add_skipped();
                 continue;
             }
@@ -320,8 +319,7 @@ extern "C" int mdc_jpeg_decode_device(mdc_ctx* c, const uint8_t* const* files, c
     if (rc == MDC_OK) {
         for (int i = 0; i < n; ++i) {
             std::string& m = msg[static_cast<size_t>(i)];
-            if (m.empty() && st[i] != kStatusOk) m = "frame " + std::to_string(i) + ": " + kind_message(st[i]);
-            if (m.empty()) m = b.incomplete_msg[static_cast<size_t>(i)];
+            if (m.empty()) m = frame_message(st[i], "frame " + std::to_string(i), b.incomplete_msg[static_cast<size_t>(i)]);
             if (status_host) status_host[i] = m.empty() ? MDC_OK : MDC_ERR_FORMAT;
             if (!m.empty() && first_bad < 0) { first_bad = i; first_msg = m; }
         }
@@ -375,14 +373,7 @@ void read_feed_frame(const mdc_seq* s, int id, int w, int h, FeedFrame& ff, mdc_
         } else {
             if (!mdc_decode_gray_image(ff.file, name, &img)) { ff.msg = mdc_last_error(); return; }
             fw = img.cols; fh = img.rows;
-            const size_t npx = static_cast<size_t>(fw) * fh;
-            if (img.depth == 8) {
-                ff.px.swap(img.px);
-            } else {                          // 16-bit: the high byte, as mdc_seq_read_gray8
-                ff.px.resize(npx);
-                const uint16_t* src = reinterpret_cast<const uint16_t*>(img.px.data());
-                for (size_t p = 0; p < npx; ++p) ff.px[p] = static_cast<uint8_t>(src[p] >> 8);
-            }
+            mdc_gray_to_u8(img, &ff.px);
         }
     } catch (const std::exception& e) {
         ff.jpeg = false;
@@ -391,12 +382,10 @@ void read_feed_frame(const mdc_seq* s, int id, int w, int h, FeedFrame& ff, mdc_
     }
     ff.w = fw; ff.h = fh;
     ff.status = MDC_OK;
-    if (fw != w || fh != h) {                 // BenchmarkDatasetReader.h:194-199
-        char msg[256];
-        snprintf(msg, sizeof msg, "expected image dimensions %d x %d; found %d x %d (image %s)", w, h, fw, fh, name.c_str());
+    if (fw != w || fh != h) {
         ff.jpeg = false;
         ff.status = MDC_ERR_INVALID_ARG;
-        ff.msg = msg;
+        ff.msg = mdc_dims_message(w, h, fw, fh, "image " + name);
     }
 }
 
@@ -422,43 +411,16 @@ int run_device_feed(const mdc_seq* s, const int* ids, int count, int w, int h, i
     std::lock_guard<std::mutex> feed_lock(mdc_seq_feed_mutex(s));
     mdc_seq_feed_stage* stage = mdc_seq_device_stage(s);
 
-    const int n_chunks = (count + chunk - 1) / chunk;
-    const int workers = std::min(threads, std::min(count, chunk));
-    std::vector<FeedFrame> frames[2];
+    std::vector<FeedFrame> frames[2];        // the two slots of the pool
     for (int b = 0; b < 2; ++b) frames[b].resize(static_cast<size_t>(std::min(chunk, count)));
-    std::mutex mu;
-    std::condition_variable cv;
-    std::vector<int> decoded(static_cast<size_t>(n_chunks), 0);
-    std::vector<std::atomic<int>> next_frame(static_cast<size_t>(n_chunks));
-    for (auto& a : next_frame) a.store(0, std::memory_order_relaxed);
-    int released = 1;                 // chunks whose frame slots may be written: 0 .. released
-    bool abort = false;
-    auto worker = [&](int) {
-        mdc_gray_image img;
-        for (int k = 0; k < n_chunks; ++k) {
-            {
-                std::unique_lock<std::mutex> lk(mu);
-                cv.wait(lk, [&] { return abort || k <= released; });
-                if (abort) return;
-            }
-            const int f0 = k * chunk, n = std::min(chunk, count - f0);
-            for (int i; (i = next_frame[static_cast<size_t>(k)].fetch_add(1, std::memory_order_relaxed)) < n;)
-                read_feed_frame(s, ids[f0 + i], w, h, frames[k & 1][static_cast<size_t>(i)], img);
-            std::lock_guard<std::mutex> lk(mu);
-            ++decoded[static_cast<size_t>(k)];
-            cv.notify_all();
-        }
-    };
-    std::vector<std::thread> pool;
-    try {
-        for (int t = 0; t < workers; ++t) pool.emplace_back(worker, t);
-    } catch (const std::exception& e) {
-        { std::lock_guard<std::mutex> lk(mu); abort = true; }
-        cv.notify_all();
-        for (auto& th : pool) th.join();
-        mdc_set_error("%s: cannot start decode threads (%s)", who, e.what());
-        return MDC_ERR_IO;
-    }
+    std::vector<mdc_gray_image> img;         // per worker
+    mdc_feed_pool pool(count, chunk, threads, [&](int t, int k, int i) {
+        read_feed_frame(s, ids[k * chunk + i], w, h, frames[k & 1][static_cast<size_t>(i)], img[static_cast<size_t>(t)]);
+        return true;
+    });
+    img.resize(static_cast<size_t>(pool.workers()));
+    if (pool.start(who) != MDC_OK) return MDC_ERR_IO;
+    const int n_chunks = pool.chunks();
 
     HostBatch batch[2];
     FeedChunk done[2];                // the host side of each slot's chunk, kept after its frame slots are handed to chunk k + 2
@@ -506,9 +468,7 @@ int run_device_feed(const mdc_seq* s, const int* ids, int count, int w, int h, i
         // the slot's previous chunk (k - 2) has left the staging buffer and the device buffers behind
         CU_CHECK(cudaEventSynchronize(ev_done[b]));
         if (stage->bytes[b] < need) {
-            if (stage->pinned[b]) mdc_host_free(stage->pinned[b]);
-            stage->pinned[b] = nullptr;
-            stage->bytes[b] = 0;
+            stage->free_slot(b);
             if (mdc_host_alloc(&stage->pinned[b], need + need / 8) != MDC_OK) return MDC_ERR_CUDA;
             stage->bytes[b] = need + need / 8;
         }
@@ -538,9 +498,7 @@ int run_device_feed(const mdc_seq* s, const int* ids, int count, int w, int h, i
         CU_CHECK(cudaEventSynchronize(ev_status[b]));
         for (int i = 0; i < fc.n; ++i) {
             if (fc.status[static_cast<size_t>(i)] != MDC_OK) continue;
-            std::string m;
-            if (status_pinned[b][i] != kStatusOk) m = std::string(mdc_seq_name(s, ids[fc.f0 + i])) + ": " + kind_message(status_pinned[b][i]);
-            else m = batch[b].incomplete_msg[static_cast<size_t>(i)];
+            std::string m = frame_message(status_pinned[b][i], mdc_seq_name(s, ids[fc.f0 + i]), batch[b].incomplete_msg[static_cast<size_t>(i)]);
             if (m.empty()) continue;
             fc.status[static_cast<size_t>(i)] = MDC_ERR_FORMAT;
             fc.sizes[2 * static_cast<size_t>(i)] = fc.sizes[2 * static_cast<size_t>(i) + 1] = 0;
@@ -552,25 +510,12 @@ int run_device_feed(const mdc_seq* s, const int* ids, int count, int w, int h, i
         return MDC_OK;
     };
     for (int k = 0; k < n_chunks && rc == MDC_OK; ++k) {
-        {
-            std::unique_lock<std::mutex> lk(mu);
-            cv.wait(lk, [&] { return decoded[static_cast<size_t>(k)] == workers; });
-        }
+        pool.wait(k);
         rc = submit(k);
-        {
-            std::lock_guard<std::mutex> lk(mu);
-            released = k + 2;             // frames[k & 1] is packed: chunk k + 2 may be read into it
-        }
-        cv.notify_all();
+        pool.release(k);              // frames[k & 1] is packed: chunk k + 2 may be read into it
         if (rc == MDC_OK && k > 0) rc = finish(k - 1);          // overlaps chunk k's J1 / J2 on the GPU
         if (rc == MDC_OK && k == n_chunks - 1) rc = finish(k);
     }
-    {
-        std::lock_guard<std::mutex> lk(mu);
-        abort = true;
-    }
-    cv.notify_all();
-    for (auto& th : pool) th.join();
     const cudaError_t drained = cudaStreamSynchronize(st);
     if (rc == MDC_OK && drained != cudaSuccess) { mdc_set_error("%s: %s", who, cudaGetErrorString(drained)); rc = MDC_ERR_CUDA; }
     for (int b = 0; b < 2; ++b) {
@@ -591,35 +536,15 @@ extern "C" int mdc_seq_prepare_device(mdc_ctx* c, const mdc_seq* s, int first, i
 extern "C" int mdc_seq_prepare_device_ex(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned flags, int out_type,
                                          void* const* d_out_levels, int levels, int threads, mdc_stream stream) {
     if (mdc_check_out_type(out_type, "mdc_seq_prepare_device") != MDC_OK) return MDC_ERR_INVALID_ARG;
-    // the argument checks of mdc_seq_prepare, in the same order
-    if (!s || !d_out_levels) { mdc_set_error("mdc_seq_prepare_device: bad argument"); return MDC_ERR_INVALID_ARG; }
-    const int n_files = mdc_seq_num_images(s);
-    if (first < 0 || count < 0 || first > n_files || count > n_files - first) {
-        mdc_set_error("mdc_seq_prepare_device: frames first = %d, count = %d outside the sequence's %d", first, count, n_files);
-        return MDC_ERR_INVALID_ARG;
-    }
-    if (levels < 1 || levels > MDC_MAX_PYR_LEVELS) {
-        mdc_set_error("mdc_seq_prepare_device: %d pyramid levels (1..%d)", levels, MDC_MAX_PYR_LEVELS);
-        return MDC_ERR_INVALID_ARG;
-    }
-    if (!c) { mdc_set_error("mdc_seq_prepare_device: bad argument"); return MDC_ERR_INVALID_ARG; }
-    int in_w = 0, in_h = 0, out_w = 0, out_h = 0;
-    mdc_ctx_geometry(c, &in_w, &in_h, &out_w, &out_h);
-    if (in_w < 1 || in_h < 1) { mdc_set_error("mdc_seq_prepare_device: context has no image geometry"); return MDC_ERR_INVALID_OBJECT; }
-    const bool rectify = (flags & MDC_RECTIFY) != 0;
-    std::vector<size_t> level_px(static_cast<size_t>(levels));
-    for (int l = 0; l < levels; ++l) {
-        level_px[static_cast<size_t>(l)] = static_cast<size_t>((rectify ? out_w : in_w) >> l) * static_cast<size_t>((rectify ? out_h : in_h) >> l);
-        if (!d_out_levels[l] && level_px[static_cast<size_t>(l)] > 0) {
-            mdc_set_error("mdc_seq_prepare_device: output level %d is NULL", l);
-            return MDC_ERR_INVALID_ARG;
-        }
-    }
-    if (count == 0) return MDC_OK;
+    int in_w = 0, in_h = 0;
+    size_t level_px[MDC_MAX_PYR_LEVELS];
+    const int checked = mdc_seq_check_prepare(c, s, first, count, flags, d_out_levels, levels, "mdc_seq_prepare_device", &in_w, &in_h, level_px);
+    if (checked != MDC_OK || count == 0) return checked;
     if (threads < 1) threads = mdc_seq_default_threads();
     CU_CHECK(cudaSetDevice(mdc_ctx_device_ordinal(c)));
     cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : static_cast<cudaStream_t>(mdc_ctx_stream_handle(c));
     // rows padded to 16 bytes keep K1 on its TMA loader; padded rows exist in rectifying mode only (mdc_prepare_batch_pitched)
+    const bool rectify = (flags & MDC_RECTIFY) != 0;
     const size_t pitch = rectify ? (static_cast<size_t>(in_w) + 15) / 16 * 16 : static_cast<size_t>(in_w);
     std::vector<int> ids(static_cast<size_t>(count));
     for (int i = 0; i < count; ++i) ids[static_cast<size_t>(i)] = first + i;
@@ -628,11 +553,8 @@ extern "C" int mdc_seq_prepare_device_ex(mdc_ctx* c, const mdc_seq* s, int first
     auto prepare = [&](const FeedChunk& fc) -> int {
         for (int i = 0; i < fc.n; ++i)
             if (fc.status[static_cast<size_t>(i)] != MDC_OK) { fail_msg = fc.msg[static_cast<size_t>(i)]; return MDC_ERR_FORMAT; }
-        std::vector<void*> outs(static_cast<size_t>(levels));
-        const size_t esize = mdc_out_elem_size(out_type);
-        for (int l = 0; l < levels; ++l)
-            outs[static_cast<size_t>(l)] = d_out_levels[l] ? static_cast<uint8_t*>(d_out_levels[l]) + static_cast<size_t>(fc.f0) * level_px[static_cast<size_t>(l)] * esize : nullptr;
-        return mdc_prepare_batch_ex(c, fc.frames, pitch, fc.n, flags, out_type, outs.data(), levels, st);
+        return mdc_prepare_batch_ex(c, fc.frames, pitch, fc.n, flags, out_type, mdc_seq_chunk_levels(d_out_levels, levels, level_px, out_type, fc.f0).data(),
+                                    levels, st);
     };
     const int rc = run_device_feed(s, ids.data(), count, in_w, in_h, threads, nullptr, pitch, st, prepare, "mdc_seq_prepare_device");
     if (rc == MDC_ERR_FORMAT) {

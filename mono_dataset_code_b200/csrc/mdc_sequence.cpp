@@ -4,19 +4,17 @@
 //   mdc_seq_open      images/ folder (sorted) or, if that is empty, images.zip (central directory, sorted names); times.txt
 //   mdc_seq_read_gray8 getImageRaw_internal with CV_LOAD_IMAGE_GRAYSCALE: 8/16-bit grey PNG (16 -> 8 bit by dropping the low byte, as
 //                     OpenCV's reader does), binary PGM, baseline JPEG (mdc_jpeg.cpp) - the same bytes as cv::imread returns.
-//   mdc_seq_prepare   getImage for a range of frames: worker threads decode chunk k+1 (two frames per thread, 16..256 frames) into
-//                     pinned memory while chunk k goes through mdc_prepare_batch_host (H2D, fused kernel, D2H on three streams).
+//   mdc_seq_prepare   getImage for a range of frames: the decode-ahead pool (mdc_feed.h) decodes chunk k+1 (two frames per thread,
+//                     16..256 frames) into pinned memory while chunk k goes through mdc_prepare_batch_host (H2D, K1, D2H).
 //
 // The zip reader handles what `zip` / Python's zipfile / the TUM archives produce: stored and deflated entries, no encryption,
 // no zip64 (archives < 4 GB, < 65535 entries), CRC-32 verified.
 #include <algorithm>
-#include <atomic>
 #include <exception>
 #include <cstdio>
 #include <cstring>
 #include <dirent.h>
 #include <fstream>
-#include <condition_variable>
 #include <mutex>
 #include <string>
 #include <sched.h>
@@ -29,6 +27,7 @@
 #include <zlib.h>
 
 #include "mdc_b200.h"
+#include "mdc_feed.h"
 #include "mdc_internal.h"
 
 namespace {
@@ -59,12 +58,11 @@ struct mdc_seq {
     std::vector<ZipEntry> entries;     // parallel to files when zipped
     std::vector<double> timestamps;
     std::vector<float> exposures;
-    // pinned staging buffers of the decode-ahead feed, kept between mdc_seq_prepare calls (pinning hundreds of MB costs tens of
-    // milliseconds — more than decoding the frames of a short call); one feed at a time per sequence object
-    mutable void* stage[2] = {nullptr, nullptr};
-    mutable size_t stage_bytes = 0;
+    // pinned staging of the host feed (mdc_seq_prepare) and of the device feed (mdc_seq_prepare_device, mdc_jpeg_gpu.cu), kept
+    // between calls (pinning hundreds of MB costs tens of milliseconds — more than decoding the frames of a short call); one feed at
+    // a time per sequence object
+    mutable mdc_seq_feed_stage host_stage, device_stage;
     mutable std::mutex feed_mutex;
-    mutable mdc_seq_feed_stage device_stage;      // the same for mdc_seq_prepare_device (mdc_jpeg_gpu.cu)
 };
 
 namespace {
@@ -180,7 +178,7 @@ void load_times(mdc_seq* s) {
     }
 }
 
-// 8-bit grey pixels of frame `id` (decoded); 16-bit sources keep the high byte
+// 8-bit grey pixels of frame `id` (decoded)
 bool read_gray8_unguarded(const mdc_seq* s, int id, std::vector<uint8_t>* px, int* w, int* h) {
     // per-thread scratch (file bytes, decoded image): no multi-megabyte allocation per frame, see mdc_jpeg.cpp
     static thread_local mdc_gray_image img;
@@ -191,12 +189,8 @@ bool read_gray8_unguarded(const mdc_seq* s, int id, std::vector<uint8_t>* px, in
     } else if (!mdc_read_gray_image(s->files[static_cast<size_t>(id)], &img)) {
         return false;
     }
-    const size_t n = static_cast<size_t>(img.rows) * img.cols;
     *w = img.cols; *h = img.rows;
-    if (img.depth == 8) { px->swap(img.px); return true; }
-    px->resize(n);
-    const uint16_t* src = reinterpret_cast<const uint16_t*>(img.px.data());
-    for (size_t i = 0; i < n; ++i) (*px)[i] = static_cast<uint8_t>(src[i] >> 8);
+    mdc_gray_to_u8(img, px);
     return true;
 }
 // no exception (bad_alloc / length_error on a hostile file) may cross the C ABI or a std::async worker
@@ -219,6 +213,18 @@ bool mdc_seq_read_file(const mdc_seq* s, int id, std::vector<uint8_t>* file) {
         mdc_set_error("%s: cannot read (%s)", s->files[static_cast<size_t>(id)].c_str(), e.what());
         return false;
     }
+}
+void mdc_gray_to_u8(mdc_gray_image& img, std::vector<uint8_t>* px) {
+    if (img.depth == 8) { px->swap(img.px); return; }
+    const size_t n = static_cast<size_t>(img.rows) * img.cols;
+    px->resize(n);
+    const uint16_t* src = reinterpret_cast<const uint16_t*>(img.px.data());
+    for (size_t i = 0; i < n; ++i) (*px)[i] = static_cast<uint8_t>(src[i] >> 8);
+}
+std::string mdc_dims_message(int w, int h, int fw, int fh, const std::string& what) {
+    char msg[256];
+    snprintf(msg, sizeof msg, "expected image dimensions %d x %d; found %d x %d (%s)", w, h, fw, fh, what.c_str());
+    return msg;
 }
 std::mutex& mdc_seq_feed_mutex(const mdc_seq* s) { return s->feed_mutex; }
 mdc_seq_feed_stage* mdc_seq_device_stage(const mdc_seq* s) { return &s->device_stage; }
@@ -257,8 +263,7 @@ extern "C" int mdc_seq_open(const char* folder, mdc_seq** out) {
 
 extern "C" void mdc_seq_close(mdc_seq* s) {
     if (!s) return;
-    for (int b = 0; b < 2; ++b) if (s->stage[b]) mdc_host_free(s->stage[b]);
-    for (int b = 0; b < 2; ++b) if (s->device_stage.pinned[b]) mdc_host_free(s->device_stage.pinned[b]);
+    for (int b = 0; b < 2; ++b) { s->host_stage.free_slot(b); s->device_stage.free_slot(b); }
     if (s->zip_fd >= 0) close(s->zip_fd);
     delete s;
 }
@@ -301,6 +306,41 @@ int mdc_seq_default_threads() {
     return n;
 }
 
+int mdc_seq_check_prepare(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned flags, void* const* out_levels, int levels,
+                          const char* who, int* in_w, int* in_h, size_t level_px[MDC_MAX_PYR_LEVELS]) {
+    if (!s || !out_levels) { mdc_set_error("%s: bad argument", who); return MDC_ERR_INVALID_ARG; }
+    const int n_files = static_cast<int>(s->files.size());
+    if (first < 0 || count < 0 || first > n_files || count > n_files - first) {      // first + count can overflow
+        mdc_set_error("%s: frames first = %d, count = %d outside the sequence's %d", who, first, count, n_files);
+        return MDC_ERR_INVALID_ARG;
+    }
+    if (levels < 1 || levels > MDC_MAX_PYR_LEVELS) {
+        mdc_set_error("%s: %d pyramid levels (1..%d)", who, levels, MDC_MAX_PYR_LEVELS);
+        return MDC_ERR_INVALID_ARG;
+    }
+    if (!c) { mdc_set_error("%s: bad argument", who); return MDC_ERR_INVALID_ARG; }
+    int out_w = 0, out_h = 0;
+    mdc_ctx_geometry(c, in_w, in_h, &out_w, &out_h);
+    if (*in_w < 1 || *in_h < 1) { mdc_set_error("%s: context has no image geometry", who); return MDC_ERR_INVALID_OBJECT; }
+    const bool rectify = (flags & MDC_RECTIFY) != 0;
+    for (int l = 0; l < levels; ++l) {      // level l of getImage's result: (w >> l) x (h >> l), mdc_prepare_batch
+        level_px[l] = static_cast<size_t>((rectify ? out_w : *in_w) >> l) * static_cast<size_t>((rectify ? out_h : *in_h) >> l);
+        if (!out_levels[l] && level_px[l] > 0) {      // a level without pixels may be NULL, as for mdc_prepare_batch
+            mdc_set_error("%s: output level %d is NULL", who, l);
+            return MDC_ERR_INVALID_ARG;
+        }
+    }
+    return MDC_OK;
+}
+
+std::vector<void*> mdc_seq_chunk_levels(void* const* out_levels, int levels, const size_t* level_px, int out_type, int f0) {
+    std::vector<void*> outs(static_cast<size_t>(levels));
+    const size_t esize = mdc_out_elem_size(out_type);
+    for (int l = 0; l < levels; ++l)
+        outs[static_cast<size_t>(l)] = out_levels[l] ? static_cast<uint8_t*>(out_levels[l]) + static_cast<size_t>(f0) * level_px[l] * esize : nullptr;
+    return outs;
+}
+
 // getImage(id, ...) for ids [first, first+count): decode ahead on `threads` host threads, prepare on the GPU chunk by chunk.
 namespace {
 int prepare_host_f32(mdc_ctx* c, const uint8_t* frames, int n_frames, unsigned flags, int, void* const* out_levels, int levels) {
@@ -317,135 +357,55 @@ extern "C" int mdc_seq_prepare(mdc_ctx* c, const mdc_seq* s, int first, int coun
 // mdc_seq_prepare(_ex): out_type is already checked (mdc_seq_prepare_ex, mdc_capi.cu); `prepare` takes each decoded chunk.
 int mdc_seq_prepare_feed(mdc_ctx* c, const mdc_seq* s, int first, int count, unsigned flags, int out_type, void* const* h_out_levels,
                          int levels, int threads, mdc_host_prepare_fn prepare) {
-    // Everything that does not depend on the context is checked first, and all of it before any staging or thread work.  The range
-    // test is written so that it cannot overflow (first + count can).
-    if (!s || !h_out_levels) { mdc_set_error("mdc_seq_prepare: bad argument"); return MDC_ERR_INVALID_ARG; }
-    const int n_files = static_cast<int>(s->files.size());
-    if (first < 0 || count < 0 || first > n_files || count > n_files - first) {
-        mdc_set_error("mdc_seq_prepare: frames first = %d, count = %d outside the sequence's %d", first, count, n_files);
-        return MDC_ERR_INVALID_ARG;
-    }
-    if (levels < 1 || levels > MDC_MAX_PYR_LEVELS) {
-        mdc_set_error("mdc_seq_prepare: %d pyramid levels (1..%d)", levels, MDC_MAX_PYR_LEVELS);
-        return MDC_ERR_INVALID_ARG;
-    }
-    if (!c) { mdc_set_error("mdc_seq_prepare: bad argument"); return MDC_ERR_INVALID_ARG; }
-    int in_w = 0, in_h = 0, out_w = 0, out_h = 0;
-    mdc_ctx_geometry(c, &in_w, &in_h, &out_w, &out_h);
-    if (in_w < 1 || in_h < 1) { mdc_set_error("mdc_seq_prepare: context has no image geometry"); return MDC_ERR_INVALID_OBJECT; }
-    const size_t n_in = static_cast<size_t>(in_w) * in_h;
-    const bool rectify = (flags & MDC_RECTIFY) != 0;
-    std::vector<size_t> level_px(static_cast<size_t>(levels));
-    for (int l = 0; l < levels; ++l) {      // level l of getImage's result: (w >> l) x (h >> l), mdc_prepare_batch
-        level_px[static_cast<size_t>(l)] = static_cast<size_t>((rectify ? out_w : in_w) >> l) * static_cast<size_t>((rectify ? out_h : in_h) >> l);
-        if (!h_out_levels[l] && level_px[static_cast<size_t>(l)] > 0) {      // a level without pixels may be NULL, as for mdc_prepare_batch
-            mdc_set_error("mdc_seq_prepare: output level %d is NULL", l);
-            return MDC_ERR_INVALID_ARG;
-        }
-    }
-    if (count == 0) return MDC_OK;
+    int in_w = 0, in_h = 0;
+    size_t level_px[MDC_MAX_PYR_LEVELS];
+    const int checked = mdc_seq_check_prepare(c, s, first, count, flags, h_out_levels, levels, "mdc_seq_prepare", &in_w, &in_h, level_px);
+    if (checked != MDC_OK || count == 0) return checked;
     if (threads < 1) threads = mdc_seq_default_threads();
-    // a chunk is what the GPU side takes at a time: two frames per decode thread (handed out dynamically, so a slow frame or a
-    // descheduled thread does not hold the chunk up), small enough that the un-overlapped head (first decode) and tail (last
-    // H2D / K1 / D2H) of a call stay short
+    // a chunk is what the GPU side takes at a time: two frames per decode thread, small enough that the un-overlapped head (first
+    // decode) and tail (last H2D / K1 / D2H) of a call stay short
     const int chunk = std::min(256, std::max(16, 2 * threads));
     std::lock_guard<std::mutex> feed_lock(s->feed_mutex);
-    const size_t need = static_cast<size_t>(chunk) * n_in;
-    if (s->stage_bytes < need) {
-        for (int b = 0; b < 2; ++b) { if (s->stage[b]) mdc_host_free(s->stage[b]); s->stage[b] = nullptr; }
-        s->stage_bytes = 0;
+    const size_t n_in = static_cast<size_t>(in_w) * in_h, need = static_cast<size_t>(chunk) * n_in;
+    mdc_seq_feed_stage& stage = s->host_stage;
+    if (stage.bytes[0] < need) {      // both slots have one size
+        for (int b = 0; b < 2; ++b) stage.free_slot(b);
         for (int b = 0; b < 2; ++b)
-            if (mdc_host_alloc(&s->stage[b], need) != MDC_OK) {
-                if (s->stage[0]) mdc_host_free(s->stage[0]);
-                s->stage[0] = s->stage[1] = nullptr;
-                return MDC_ERR_CUDA;
-            }
-        s->stage_bytes = need;
+            if (mdc_host_alloc(&stage.pinned[b], need) != MDC_OK) { stage.free_slot(0); stage.pinned[1] = nullptr; return MDC_ERR_CUDA; }
+        stage.bytes[0] = stage.bytes[1] = need;
     }
-    void* const stage[2] = {s->stage[0], s->stage[1]};
 
-    // Decode pool: `threads` workers live for the whole call.  The workers take the frames of chunk k one by one (an atomic counter per
-    // chunk) and decode them into stage[k & 1], then move on to chunk k+1 as soon as the GPU side has released that chunk's buffer
-    // (chunk k-1 consumed), so decode of chunk k+1 overlaps H2D / K1 / D2H of chunk k, and nobody creates multi-megabyte buffers per frame.
-    const int n_chunks = (count + chunk - 1) / chunk;
-    const int workers = std::min(threads, std::min(count, chunk));
-    std::mutex mu;
-    std::condition_variable cv;
-    std::vector<int> decoded(static_cast<size_t>(n_chunks), 0);      // workers finished with chunk k
-    std::vector<std::atomic<int>> next_frame(static_cast<size_t>(n_chunks));      // next frame of chunk k nobody has taken yet
-    for (auto& a : next_frame) a.store(0, std::memory_order_relaxed);
-    int released = 1;                 // chunks whose buffer may be written: 0 .. released (stage[0] and stage[1] are free at the start)
-    bool abort = false;
-    // first error met in chunk k.  Per chunk, because the workers run one chunk ahead: an error in chunk k+1 must not stop the call
-    // before chunk k, which decoded fine, has been prepared (the reference prepares every frame before the bad one).
-    std::vector<std::string> chunk_error(static_cast<size_t>(n_chunks));
-    auto worker = [&](int) {
-        std::vector<uint8_t> px;
-        for (int k = 0; k < n_chunks; ++k) {
-            {
-                std::unique_lock<std::mutex> lk(mu);
-                cv.wait(lk, [&] { return abort || k <= released; });
-                if (abort) return;
-            }
-            const int f0 = k * chunk, n = std::min(chunk, count - f0);
-            uint8_t* dst = static_cast<uint8_t*>(stage[k & 1]);
-            std::string err;
-            for (int i; err.empty() && (i = next_frame[static_cast<size_t>(k)].fetch_add(1, std::memory_order_relaxed)) < n;) {
-                int w = 0, h = 0;
-                if (!read_gray8(s, first + f0 + i, &px, &w, &h)) err = mdc_last_error();
-                else if (w != in_w || h != in_h) {      // BenchmarkDatasetReader.h:194-199
-                    char msg[256];
-                    snprintf(msg, sizeof msg, "expected image dimensions %d x %d; found %d x %d (image %s)", in_w, in_h, w, h, s->files[static_cast<size_t>(first + f0 + i)].c_str());
-                    err = msg;
-                } else {
-                    memcpy(dst + static_cast<size_t>(i) * n_in, px.data(), n_in);
-                }
-            }
-            std::lock_guard<std::mutex> lk(mu);
-            if (!err.empty() && chunk_error[static_cast<size_t>(k)].empty()) chunk_error[static_cast<size_t>(k)] = err;
-            ++decoded[static_cast<size_t>(k)];
-            cv.notify_all();
-        }
-    };
-    std::vector<std::thread> pool;
-    try {
-        for (int t = 0; t < workers; ++t) pool.emplace_back(worker, t);
-    } catch (const std::exception& e) {
-        { std::lock_guard<std::mutex> lk(mu); abort = true; }
-        cv.notify_all();
-        for (auto& th : pool) th.join();
-        mdc_set_error("mdc_seq_prepare: cannot start decode threads (%s)", e.what());
-        return MDC_ERR_IO;
-    }
-    int rc = MDC_OK;
-    for (int k = 0; k < n_chunks && rc == MDC_OK; ++k) {
-        std::string err;
-        {
-            std::unique_lock<std::mutex> lk(mu);
-            cv.wait(lk, [&] { return decoded[static_cast<size_t>(k)] == workers; });
-            err = chunk_error[static_cast<size_t>(k)];
-        }
-        if (!err.empty()) {
-            printf("ERROR: %s\n", err.c_str());
-            mdc_set_error("mdc_seq_prepare: %s", err.c_str());
-            rc = MDC_ERR_FORMAT;
-            break;
-        }
+    // chunk k is decoded into stage slot k & 1 while chunk k - 1 is prepared.  A frame's error is kept per frame (each frame is read
+    // by one worker): an error in chunk k+1 must not stop the call before chunk k, which decoded fine, has been prepared (the
+    // reference prepares every frame before the bad one).  A worker takes no further frame of a chunk after an error in it.
+    std::vector<std::string> frame_error(static_cast<size_t>(count));
+    std::vector<std::vector<uint8_t>> px;      // per worker
+    mdc_feed_pool pool(count, chunk, threads, [&](int t, int k, int i) {
+        const int f = k * chunk + i;
+        std::vector<uint8_t>& p = px[static_cast<size_t>(t)];
+        std::string& err = frame_error[static_cast<size_t>(f)];
+        int w = 0, h = 0;
+        if (!read_gray8(s, first + f, &p, &w, &h)) err = mdc_last_error();
+        else if (w != in_w || h != in_h) err = mdc_dims_message(in_w, in_h, w, h, "image " + s->files[static_cast<size_t>(first + f)]);
+        else memcpy(static_cast<uint8_t*>(stage.pinned[k & 1]) + static_cast<size_t>(i) * n_in, p.data(), n_in);
+        return err.empty();
+    });
+    px.resize(static_cast<size_t>(pool.workers()));
+    if (pool.start("mdc_seq_prepare") != MDC_OK) return MDC_ERR_IO;
+    for (int k = 0; k < pool.chunks(); ++k) {
+        pool.wait(k);
         const int f0 = k * chunk, n = std::min(chunk, count - f0);
-        std::vector<void*> outs(static_cast<size_t>(levels));
-        const size_t esize = mdc_out_elem_size(out_type);
-        for (int l = 0; l < levels; ++l)
-            outs[static_cast<size_t>(l)] = h_out_levels[l] ? static_cast<uint8_t*>(h_out_levels[l]) + static_cast<size_t>(f0) * level_px[static_cast<size_t>(l)] * esize : nullptr;
-        rc = prepare(c, static_cast<const uint8_t*>(stage[k & 1]), n, flags, out_type, outs.data(), levels);      // returns after the D2H copy
-        std::lock_guard<std::mutex> lk(mu);
-        released = k + 2;             // stage[k & 1] is free again: chunk k+2 may be decoded into it
-        cv.notify_all();
+        const auto chunk_end = frame_error.begin() + f0 + n;
+        const auto bad = std::find_if(chunk_end - n, chunk_end, [](const std::string& e) { return !e.empty(); });      // its lowest bad frame
+        if (bad != chunk_end) {
+            printf("ERROR: %s\n", bad->c_str());
+            mdc_set_error("mdc_seq_prepare: %s", bad->c_str());
+            return MDC_ERR_FORMAT;
+        }
+        const int rc = prepare(c, static_cast<const uint8_t*>(stage.pinned[k & 1]), n, flags, out_type,
+                               mdc_seq_chunk_levels(h_out_levels, levels, level_px, out_type, f0).data(), levels);      // returns after the D2H copy
+        if (rc != MDC_OK) return rc;
+        pool.release(k);
     }
-    {
-        std::lock_guard<std::mutex> lk(mu);
-        abort = true;                 // error path: wake workers that wait for a buffer that will not be released
-    }
-    cv.notify_all();
-    for (auto& th : pool) th.join();
-    return rc;
+    return MDC_OK;
 }
