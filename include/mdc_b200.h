@@ -437,6 +437,48 @@ int mdc_rc_gstep(mdc_ctx* c, const uint8_t* d_data, int n, int npix, const doubl
 int mdc_rc_rescale(mdc_ctx* c, int npix, double* d_E, double* d_G, double* factor_host);
 int mdc_rc_rmse(mdc_ctx* c, const uint8_t* d_data, int n, int npix, const double* d_t, const double* d_G, const double* d_E, double out_host[2]);
 int mdc_response_calib(mdc_ctx* c, const uint8_t* d_data, int n, int npix, const double* d_t, int nits, double* d_E, double* d_G, double* log_host);
+/* mdc_response_calib with a per-step hook: step(iteration, which, d_E, d_G, user) is called after E-init (iteration 0,
+ * MDC_RC_STEP_E), and in iteration it = 0..nits-1 after the G-step (it + 1, MDC_RC_STEP_G) and after the E-step, before the
+ * rescale (it + 1, MDC_RC_STEP_E), each right after the rmse line of that step is printed: where the reference plots
+ * (main_responseCalib.cpp:273, :309-310, :344-345).  The context's stream is idle during the call, so the hook may enqueue work on
+ * the context (the plots below) but must not change d_E or d_G.  The loop writes d_E and d_G again on the context's stream as soon
+ * as the hook returns, without waiting for other streams: work the hook puts on another stream that reads them (a copy, a plot
+ * call with a non-NULL stream) must be finished before it returns.  step = NULL is mdc_response_calib; the hook changes no result. */
+#define MDC_RC_STEP_E 0
+#define MDC_RC_STEP_G 1
+typedef void (*mdc_rc_step_fn)(int iteration, int which, const double* d_E, const double* d_G, void* user);
+int mdc_response_calib_ex(mdc_ctx* c, const uint8_t* d_data, int n, int npix, const double* d_t, int nits, double* d_E, double* d_G,
+                          double* log_host, mdc_rc_step_fn step, void* user);
+
+/* responseCalib's result images (main_responseCalib.cpp:72-146), the pixels the reference hands to cv::imwrite, bit for bit
+ * (DEVICE pointers; log and exp are glibc's, csrc/mdc_libm.h):
+ *   mdc_rc_plot_e_range  d_range4 = {min ln(E+20), max ln(E+20), min E, max E} over npix values, with the reference's starting values
+ *                        1e10 / -1e10 and strict comparisons (NaN is skipped; all NaN or npix = 0 leaves the starting values).
+ *                        Ties go to the lower pixel index, so a zero extreme has the sign the reference's scan gives it.  The
+ *                        ranges of several slices of an image, taken in slice order, join into the range of the whole image
+ *                        with the same rule: a later slice's value replaces an earlier one only when strictly smaller / larger.
+ *   mdc_rc_plot_e_map    from a range in device memory: d_bgr [npix][3] u8, the colour map of ln(E+20) in cv::Mat's BGR order
+ *                        (E-k.png), and d_e16 [npix] u16 = 65025 (E - Emin) / (Emax - Emin) (E-k16.png), converted through a
+ *                        32-bit truncation as x86-64 converts (NaN and values of 2^31 or more give 0).  Slices concatenate.
+ *   mdc_rc_plot_e        both passes on one stream.
+ *   mdc_rc_plot_g        d_out [256][256] u8: plotG's image (G-k.png) as cv::imwrite converts GImg * 255 (round half to even,
+ *                        saturate, NaN -> 0); minmax_host (may be NULL) = {min G, max G}, the values it prints. */
+int mdc_rc_plot_e_range(mdc_ctx* c, const double* d_E, int npix, double* d_range4, mdc_stream stream);
+int mdc_rc_plot_e_map(mdc_ctx* c, const double* d_E, int npix, const double* d_range4, uint8_t* d_bgr, uint16_t* d_e16, mdc_stream stream);
+int mdc_rc_plot_e(mdc_ctx* c, const double* d_E, int npix, double* d_range4, uint8_t* d_bgr, uint16_t* d_e16, mdc_stream stream);
+int mdc_rc_plot_g(mdc_ctx* c, const double* d_G, uint8_t* d_out, double* minmax_host, mdc_stream stream);
+
+/* glibc's double exp and log as the plots evaluate them (csrc/mdc_libm.h), for checking against a deployment's libm:
+ * out[i] = op(in[i]) on the host or on the GPU (device pointers). */
+#define MDC_LIBM_EXP 0
+#define MDC_LIBM_LOG 1
+void mdc_libm_host(int op, const double* in, double* out, size_t n);
+int mdc_libm_device(int op, const double* d_in, double* d_out, size_t n, int device, mdc_stream stream);
+
+/* A PNG file of 8-bit or 16-bit samples, 1 (grey) or 3 channels, as cv::imwrite takes them: 3 channels in BGR order, 16-bit
+ * samples in host byte order; rows row_bytes apart.  Decodes to the same pixels as cv::imwrite's file.  MDC_ERR_IO when the
+ * file cannot be written. */
+int mdc_png_write(const char* path, const void* pixels, int w, int h, size_t row_bytes, int depth, int channels);
 /* The two global reductions of the loop as per-rank partials, for PIXEL-SHARDED runs (pixels are independent in every pass,
  * main_responseCalib.cpp:317-346; each rank holds its slice of every image as [n][npix_local]).  The accumulators stay on the device:
  *   mdc_rc_gstep_accumulate  d_gsum256[b] = sum E[k]*t[i], d_gnum256[b] = count over this rank's pixels (:290-299); reuse_counts != 0

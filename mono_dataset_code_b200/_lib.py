@@ -17,6 +17,10 @@ RECTIFY, REMOVE_GAMMA, REMOVE_VIGNETTE, NAN_OVEREXPOSED = 1, 2, 4, 8
 OUT_F32, OUT_F16, OUT_U8 = 0, 1, 2          # element type of prepared levels (MDC_OUT_*)
 FOV_CROP, FOV_FULL, FOV_EXPLICIT = -1, -2, 0
 MAX_PYR_LEVELS = 8
+RC_STEP_E, RC_STEP_G = 0, 1                 # which step of mdc_response_calib_ex calls back
+LIBM_EXP, LIBM_LOG = 0, 1
+# mdc_rc_step_fn: (iteration, which, d_E, d_G, user)
+RC_STEP_FN = C.CFUNCTYPE(None, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p)
 
 _f32p = C.POINTER(C.c_float)
 _vp = C.c_void_p
@@ -106,6 +110,14 @@ SIGNATURES = {
     "mdc_rc_rescale": (C.c_int, [_vp, C.c_int, _vp, _vp, C.POINTER(C.c_double)]),
     "mdc_rc_rmse": (C.c_int, [_vp, _vp, C.c_int, C.c_int, _vp, _vp, _vp, C.POINTER(C.c_double)]),
     "mdc_response_calib": (C.c_int, [_vp, _vp, C.c_int, C.c_int, _vp, C.c_int, _vp, _vp, C.POINTER(C.c_double)]),
+    "mdc_response_calib_ex": (C.c_int, [_vp, _vp, C.c_int, C.c_int, _vp, C.c_int, _vp, _vp, C.POINTER(C.c_double), _vp, _vp]),
+    "mdc_rc_plot_e_range": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp]),
+    "mdc_rc_plot_e_map": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp, _vp, _vp]),
+    "mdc_rc_plot_e": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp, _vp, _vp]),
+    "mdc_rc_plot_g": (C.c_int, [_vp, _vp, _vp, C.POINTER(C.c_double), _vp]),
+    "mdc_libm_host": (None, [C.c_int, _vp, _vp, C.c_size_t]),
+    "mdc_libm_device": (C.c_int, [C.c_int, _vp, _vp, C.c_size_t, C.c_int, _vp]),
+    "mdc_png_write": (C.c_int, [C.c_char_p, _vp, C.c_int, C.c_int, C.c_size_t, C.c_int, C.c_int]),
     "mdc_rc_gstep_accumulate": (C.c_int, [_vp, _vp, C.c_int, C.c_int, _vp, _vp, _vp, _vp, C.c_int, _vp]),
     "mdc_rc_gstep_finish": (C.c_int, [_vp, _vp, _vp, _vp, _vp]),
     "mdc_rc_gstep_scale": (C.c_int, [_vp, _vp, C.c_int, _vp, C.c_int, _vp, _vp]),

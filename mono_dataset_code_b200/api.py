@@ -429,14 +429,78 @@ class Context:
                                          C.c_void_p(G.data_ptr()), C.c_void_p(E.data_ptr()), C.c_void_p(acc.data_ptr()), self._stream(data)),
               "mdc_rc_rmse_accumulate")
 
-    def response_calib(self, data, t, nits, E, G):
-        """The optimisation loop of responseCalib's main(); returns the per-iteration log [nits, 4]."""
+    def response_calib(self, data, t, nits, E, G, on_step=None):
+        """The optimisation loop of responseCalib's main(); returns the per-iteration log [nits, 4].
+        on_step(iteration, which, E, G), if given, is called where the reference plots: after E-init (0, "E"), and in iteration it
+        after the G-step (it + 1, "G") and after the E-step, before the rescale (it + 1, "E").  E and G hold that step's values; the
+        callback may read them, copy them or run the plots on them (rc_plot_e, rc_plot_g) but must not change them.  Work it enqueues
+        on torch's current stream is finished before the loop goes on (the loop writes E and G in place on the context's own stream),
+        so a snapshot such as E.clone() holds that step's values."""
         self._drain(data)
         log = np.zeros((max(nits, 1), 4), np.float64)
-        check(lib.mdc_response_calib(self._h, C.c_void_p(data.data_ptr()), data.shape[0], data.shape[1], C.c_void_p(t.data_ptr()), nits,
-                                     C.c_void_p(E.data_ptr()), C.c_void_p(G.data_ptr()), log.ctypes.data_as(C.POINTER(C.c_double))),
-              "mdc_response_calib")
+        failed = []
+
+        def step(iteration, which, _e, _g, _user):
+            if failed:
+                return
+            try:
+                on_step(iteration, "G" if which == _lib.RC_STEP_G else "E", E, G)
+            except BaseException as exc:              # raised again below: an exception cannot cross the C frames
+                failed.append(exc)
+            finally:
+                self._drain(E)                        # the next pass overwrites E / G without waiting for torch's stream
+
+        hook = _lib.RC_STEP_FN(step) if on_step is not None else None
+        check(lib.mdc_response_calib_ex(self._h, C.c_void_p(data.data_ptr()), data.shape[0], data.shape[1], C.c_void_p(t.data_ptr()), nits,
+                                        C.c_void_p(E.data_ptr()), C.c_void_p(G.data_ptr()), log.ctypes.data_as(C.POINTER(C.c_double)),
+                                        C.cast(hook, C.c_void_p) if hook else None, None), "mdc_response_calib_ex")
+        if failed:
+            raise failed[0]
         return log[:nits]
+
+    # ---- responseCalib's result images (main_responseCalib.cpp:72-146; CUDA tensors, on torch's current stream)
+    def rc_plot_e_range(self, E, range4=None):
+        """{min ln(E+20), max ln(E+20), min E, max E} of a float64 CUDA tensor (any shape) into a float64 CUDA tensor [4] (new when
+        range4 is None).  The ranges of slices join into the range of the whole image by strict min / max taken in slice order
+        (rc_plot_join_ranges)."""
+        import torch
+        assert E.is_cuda and E.dtype == torch.float64 and E.is_contiguous()
+        range4 = torch.empty(4, dtype=torch.float64, device=E.device) if range4 is None else range4
+        assert range4.is_cuda and range4.dtype == torch.float64 and range4.numel() == 4
+        check(lib.mdc_rc_plot_e_range(self._h, C.c_void_p(E.data_ptr()), E.numel(), C.c_void_p(range4.data_ptr()), self._stream(E)),
+              "mdc_rc_plot_e_range")
+        return range4
+
+    def rc_plot_e_map(self, E, range4, bgr=None, e16=None):
+        """plotE's two images of E under the range range4 (a CUDA tensor): bgr uint8 [npix, 3] (BGR order) and e16 uint16 [npix]."""
+        import torch
+        assert E.is_cuda and E.dtype == torch.float64 and E.is_contiguous()
+        assert range4.is_cuda and range4.dtype == torch.float64 and range4.numel() == 4
+        n = E.numel()
+        bgr = torch.empty((n, 3), dtype=torch.uint8, device=E.device) if bgr is None else bgr
+        e16 = torch.empty(n, dtype=torch.uint16, device=E.device) if e16 is None else e16
+        assert bgr.is_cuda and bgr.dtype == torch.uint8 and bgr.is_contiguous() and bgr.numel() == 3 * n
+        assert e16.is_cuda and e16.dtype == torch.uint16 and e16.is_contiguous() and e16.numel() == n
+        check(lib.mdc_rc_plot_e_map(self._h, C.c_void_p(E.data_ptr()), n, C.c_void_p(range4.data_ptr()), C.c_void_p(bgr.data_ptr()),
+                                    C.c_void_p(e16.data_ptr()), self._stream(E)), "mdc_rc_plot_e_map")
+        return bgr, e16
+
+    def rc_plot_e(self, E, w, h):
+        """plotE (E-k.png, E-k16.png) of a w x h irradiance: (bgr uint8 CUDA [h, w, 3] in BGR order, e16 uint16 CUDA [h, w],
+        (min ln(E+20), max ln(E+20), min E, max E))."""
+        assert E.numel() == w * h
+        range4 = self.rc_plot_e_range(E)
+        bgr, e16 = self.rc_plot_e_map(E, range4)
+        return bgr.view(h, w, 3), e16.view(h, w), tuple(range4.tolist())
+
+    def rc_plot_g(self, G):
+        """plotG (G-k.png) of a float64 CUDA tensor [256]: (uint8 CUDA [256, 256], (min G, max G))."""
+        import torch
+        assert G.is_cuda and G.dtype == torch.float64 and G.is_contiguous() and G.numel() == 256
+        out = torch.empty((256, 256), dtype=torch.uint8, device=G.device)
+        mm = (C.c_double * 2)()
+        check(lib.mdc_rc_plot_g(self._h, C.c_void_p(G.data_ptr()), C.c_void_p(out.data_ptr()), mm, self._stream(G)), "mdc_rc_plot_g")
+        return out, (mm[0], mm[1])
 
     # ---- vignetteCalib optimiser (CUDA tensors; main_vignetteCalib.cpp:395-585)
     @staticmethod
@@ -766,6 +830,46 @@ def atanf_device(x):
     check(lib.mdc_atanf_device(C.c_void_p(x.data_ptr()), C.c_void_p(out.data_ptr()), x.numel(), x.device.index or 0,
                                C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)), "mdc_atanf_device")
     return out
+
+
+def rc_plot_join_ranges(ranges):
+    """The range of a whole image from the ranges of its pixel slices (rc_plot_e_range of each), given in slice order: strict
+    min / max from the starting values 1e10 / -1e10, so an earlier slice keeps a tie, as the reference's scan keeps the first of
+    +0 and -0.  Returns [min ln(E+20), max ln(E+20), min E, max E] as Python floats."""
+    out = [1e10, -1e10, 1e10, -1e10]
+    for r in ranges:
+        r = [float(v) for v in (r.tolist() if hasattr(r, "tolist") else r)]
+        for k in range(4):
+            if (r[k] > out[k]) if k & 1 else (r[k] < out[k]):
+                out[k] = r[k]
+    return out
+
+
+def libm_host(x: np.ndarray, op: str) -> np.ndarray:
+    """glibc's double exp or log as the plots evaluate them (csrc/mdc_libm.h), on the host; op is "exp" or "log"."""
+    x = np.ascontiguousarray(x, dtype=np.float64)
+    out = np.empty_like(x)
+    lib.mdc_libm_host(_lib.LIBM_EXP if op == "exp" else _lib.LIBM_LOG, x.ctypes.data, out.ctypes.data, x.size)
+    return out
+
+
+def libm_device(x, op: str):
+    """The same functions evaluated by the GPU (float64 CUDA tensor in, new tensor out)."""
+    import torch
+    assert x.is_cuda and x.dtype == torch.float64 and x.is_contiguous() and op in ("exp", "log")
+    out = torch.empty_like(x)
+    check(lib.mdc_libm_device(_lib.LIBM_EXP if op == "exp" else _lib.LIBM_LOG, C.c_void_p(x.data_ptr()), C.c_void_p(out.data_ptr()),
+                              x.numel(), x.device.index or 0, C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)), "mdc_libm_device")
+    return out
+
+
+def png_write(path: str, img: np.ndarray) -> None:
+    """Write a uint8 or uint16 image [h, w] (grey) or [h, w, 3] (BGR, as cv2.imwrite takes it) as a PNG file; rows may be strided."""
+    assert img.dtype in (np.uint8, np.uint16) and img.ndim in (2, 3) and (img.ndim == 2 or img.shape[2] == 3)
+    if img.strides[0] < 0 or img.strides[-1] != img.itemsize or (img.ndim == 3 and img.strides[1] != 3 * img.itemsize):
+        img = np.ascontiguousarray(img)
+    check(lib.mdc_png_write(path.encode(), img.ctypes.data, img.shape[1], img.shape[0], img.strides[0], 8 * img.itemsize,
+                            1 if img.ndim == 2 else 3), "mdc_png_write")
 
 
 class _Marker(C.Structure):

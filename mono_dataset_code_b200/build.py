@@ -41,21 +41,22 @@ def build(force: bool = False, verbose: bool = False) -> str:
     gxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"   # not $CXX: see oracle/Makefile
     inc = ["-I" + os.path.join(ROOT, "include"), "-I" + CSRC]
     headers = [os.path.join(ROOT, "include", "mdc_b200.h"), os.path.join(CSRC, "mdc_internal.h"),
-               os.path.join(CSRC, "mdc_kernels.cuh"), os.path.join(CSRC, "mdc_atanf.h"), os.path.join(CSRC, "mdc_jpeg.h"),
+               os.path.join(CSRC, "mdc_kernels.cuh"), os.path.join(CSRC, "mdc_atanf.h"), os.path.join(CSRC, "mdc_libm.h"), os.path.join(CSRC, "mdc_jpeg.h"),
                os.path.join(CSRC, "mdc_jpeg_entropy.cuh"), os.path.join(CSRC, "mdc_jpeg_encode.cuh"), os.path.join(CSRC, "mdc_feed.h"),
                os.path.abspath(__file__)]
     obj_dir = os.path.join(PKG, "build")
     os.makedirs(obj_dir, exist_ok=True)
     os.makedirs(LIB_DIR, exist_ok=True)
     objs, log, rebuilt = [], [], False
-    for src in ("mdc_host_models.cpp", "mdc_gray_image.cpp", "mdc_jpeg.cpp", "mdc_sequence.cpp", "mdc_marker.cpp"):
+    for src in ("mdc_host_models.cpp", "mdc_gray_image.cpp", "mdc_jpeg.cpp", "mdc_sequence.cpp", "mdc_marker.cpp", "mdc_png.cpp"):
         o = os.path.join(obj_dir, src + ".o")
         s = os.path.join(CSRC, src)
         if force or _newer(o, [s] + headers):
             _run([gxx, "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-Wall", *inc, "-c", s, "-o", o], log)
             rebuilt = True
         objs.append(o)
-    for src in ("mdc_kernels.cu", "mdc_capi.cu", "mdc_vignette_calib.cu", "mdc_marker.cu", "mdc_jpeg_gpu.cu", "mdc_jpeg_encode.cu"):
+    for src in ("mdc_kernels.cu", "mdc_capi.cu", "mdc_vignette_calib.cu", "mdc_marker.cu", "mdc_jpeg_gpu.cu", "mdc_jpeg_encode.cu",
+                "mdc_rc_plot.cu"):
         o = os.path.join(obj_dir, src + ".o")
         s = os.path.join(CSRC, src)
         if force or _newer(o, [s] + headers):

@@ -1269,20 +1269,31 @@ extern "C" int mdc_rc_rmse(mdc_ctx* c, const uint8_t* d_data, int n, int npix, c
 }
 
 extern "C" int mdc_response_calib(mdc_ctx* c, const uint8_t* d_data, int n, int npix, const double* d_t, int nits, double* d_E, double* d_G, double* log_host) {
+    return mdc_response_calib_ex(c, d_data, n, npix, d_t, nits, d_E, d_G, log_host, nullptr, nullptr);
+}
+
+extern "C" int mdc_response_calib_ex(mdc_ctx* c, const uint8_t* d_data, int n, int npix, const double* d_t, int nits, double* d_E, double* d_G,
+                                     double* log_host, mdc_rc_step_fn step, void* user) {
     if (!c || !d_data || !d_t || !d_E || !d_G || n < 1 || npix < 1 || nits < 0) { mdc_set_error("mdc_response_calib: bad argument"); return MDC_ERR_INVALID_ARG; }
     int rc = mdc_rc_einit(c, d_data, n, npix, d_E, c->stream);          // starting irradiance = mean of all images
     if (rc != MDC_OK) return rc;
     CU_CHECK(cudaMemsetAsync(d_G, 0, 256 * sizeof(double), c->stream));
+    if (step) {
+        CU_CHECK(cudaStreamSynchronize(c->stream));
+        step(0, MDC_RC_STEP_E, d_E, d_G, user);
+    }
     for (int it = 0; it < nits; ++it) {
         double r[2], row[4] = {0, 0, 0, 0};
         if ((rc = rc_gstep_impl(c, d_data, n, npix, d_t, d_E, d_G, /*reuse_counts=*/it > 0, c->stream)) != MDC_OK) return rc;
         if ((rc = mdc_rc_rmse(c, d_data, n, npix, d_t, d_G, d_E, r)) != MDC_OK) return rc;
         row[0] = r[0];
         printf("optG RMSE = %f! \t", r[0]);
+        if (step) step(it + 1, MDC_RC_STEP_G, d_E, d_G, user);
         if ((rc = mdc_estep(c, d_data, n, npix, d_t, d_G, d_E, c->stream)) != MDC_OK) return rc;
         if ((rc = mdc_rc_rmse(c, d_data, n, npix, d_t, d_G, d_E, r)) != MDC_OK) return rc;
         row[1] = r[0];
         printf("OptE RMSE = %f!  \t", r[0]);
+        if (step) step(it + 1, MDC_RC_STEP_E, d_E, d_G, user);
         double factor = 0;
         if ((rc = mdc_rc_rescale(c, npix, d_E, d_G, &factor)) != MDC_OK) return rc;
         if ((rc = mdc_rc_rmse(c, d_data, n, npix, d_t, d_G, d_E, r)) != MDC_OK) return rc;

@@ -23,9 +23,8 @@
 //                      [facH=5] [device=0]
 //
 // Build (see tests/test_vignette_calib_tool.py):  g++ -std=c++11 -O2 -Iinclude tools/vignetteCalib_b200.cpp
-//                                                 -Lmono_dataset_code_b200/lib -lmdc_b200 -L/usr/local/cuda/lib64 -lcudart -lz
+//                                                 -Lmono_dataset_code_b200/lib -lmdc_b200 -L/usr/local/cuda/lib64 -lcudart
 #include <cuda_runtime.h>
-#include <zlib.h>
 
 #include <algorithm>
 #include <cmath>
@@ -65,62 +64,21 @@ void parse_option(const char* arg, Options* o) {
 #define CUDA_OR_DIE(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) { printf("%s: %s\n", #expr, cudaGetErrorString(e__)); exit(2); } } while (0)
 #define MDC_OR_DIE(expr) do { int r__ = (expr); if (r__ != MDC_OK) { printf("%s failed (%d): %s\n", #expr, r__, mdc_last_error()); exit(2); } } while (0)
 
-// PNG with filter type 0 on every row: colour type 0 (grey) or 2 (RGB), 8 or 16 bits, samples big-endian
-bool write_png(const std::string& path, const std::vector<uint8_t>& rows_be, int w, int h, int depth, int colour) {
-    const size_t stride = static_cast<size_t>(w) * (colour == 2 ? 3 : 1) * (depth / 8);
-    std::vector<uint8_t> raw;
-    raw.reserve((stride + 1) * h);
-    for (int y = 0; y < h; ++y) {
-        raw.push_back(0);
-        raw.insert(raw.end(), rows_be.begin() + y * stride, rows_be.begin() + (y + 1) * stride);
-    }
-    uLongf zlen = compressBound(raw.size());
-    std::vector<uint8_t> z(zlen);
-    if (compress2(z.data(), &zlen, raw.data(), raw.size(), 6) != Z_OK) return false;
-    z.resize(zlen);
-    FILE* f = fopen(path.c_str(), "wb");
-    if (!f) return false;
-    auto be32 = [](uint8_t* p, uint32_t v) { p[0] = v >> 24; p[1] = v >> 16; p[2] = v >> 8; p[3] = v; };
-    auto chunk = [&](const char* tag, const uint8_t* data, size_t len) {
-        uint8_t head[8];
-        be32(head, static_cast<uint32_t>(len));
-        memcpy(head + 4, tag, 4);
-        uLong crc = crc32(0L, head + 4, 4);
-        if (len) crc = crc32(crc, data, static_cast<uInt>(len));
-        uint8_t tail[4];
-        be32(tail, static_cast<uint32_t>(crc));
-        fwrite(head, 1, 8, f);
-        if (len) fwrite(data, 1, len, f);
-        fwrite(tail, 1, 4, f);
-    };
-    static const uint8_t sig[8] = {0x89, 'P', 'N', 'G', '\r', '\n', 0x1a, '\n'};
-    fwrite(sig, 1, 8, f);
-    uint8_t ihdr[13];
-    be32(ihdr, w);
-    be32(ihdr + 4, h);
-    ihdr[8] = static_cast<uint8_t>(depth); ihdr[9] = static_cast<uint8_t>(colour); ihdr[10] = ihdr[11] = ihdr[12] = 0;
-    chunk("IHDR", ihdr, 13);
-    chunk("IDAT", z.data(), z.size());
-    chunk("IEND", nullptr, 0);
-    return fclose(f) == 0;
-}
-
 // cv::Mat(CV_32F) * 254.9 * 254.9 -> convertTo(CV_16U) (:570-581): two float products, then round to nearest even and saturate
 // (NaN -> 0)
 bool write_vignette_png(const std::string& path, const std::vector<float>& v, int w, int h) {
-    std::vector<uint8_t> px(v.size() * 2);
+    std::vector<uint16_t> px(v.size());
     for (size_t i = 0; i < v.size(); ++i) {
         float a = static_cast<float>(v[i] * 254.9);
         a = static_cast<float>(a * 254.9);
         const double r = nearbyint(static_cast<double>(a));
         const unsigned u = r > 65535 ? 65535u : (r > 0 ? static_cast<unsigned>(r) : 0u);
-        px[2 * i] = static_cast<uint8_t>(u >> 8);
-        px[2 * i + 1] = static_cast<uint8_t>(u);
+        px[i] = static_cast<uint16_t>(u);
     }
-    return write_png(path, px, w, h, 16, 0);
+    return mdc_png_write(path.c_str(), px.data(), w, h, 2 * static_cast<size_t>(w), 16, 1) == MDC_OK;
 }
 
-// displayImage (:72-93): grey 255*(I-vmin)/(vmax-vmin) truncated to 8 bits; NaN is the Mat's BGR (0,0,255), i.e. red
+// displayImage (:72-93): grey 255*(I-vmin)/(vmax-vmin) truncated to 8 bits; NaN is BGR (0,0,255), i.e. red
 bool write_plane_png(const std::string& path, const std::vector<float>& I, int w, int h) {
     float vmin = 1e10, vmax = -1e10;
     for (float v : I) {
@@ -131,11 +89,11 @@ bool write_plane_png(const std::string& path, const std::vector<float>& I, int w
     std::vector<uint8_t> px(I.size() * 3);
     for (size_t i = 0; i < I.size(); ++i) {
         uint8_t* p = &px[3 * i];
-        if (std::isnan(I[i])) { p[0] = 255; p[1] = 0; p[2] = 0; continue; }
+        if (std::isnan(I[i])) { p[0] = 0; p[1] = 0; p[2] = 255; continue; }
         const float c = 255 * (I[i] - vmin) / (vmax - vmin);
         p[0] = p[1] = p[2] = c >= 0 && c < 256 ? static_cast<uint8_t>(c) : (c >= 256 ? 255 : 0);
     }
-    return write_png(path, px, w, h, 8, 2);
+    return mdc_png_write(path.c_str(), px.data(), w, h, 3 * static_cast<size_t>(w), 8, 3) == MDC_OK;
 }
 
 // Every skip-th frame (ids) decoded into the device stack d_stack [ids][hI][pitch] in one call; exits at the first one that cannot be
