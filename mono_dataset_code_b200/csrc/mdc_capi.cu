@@ -12,6 +12,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <tuple>
 #include <utility>
 #include <vector>
 
@@ -49,11 +50,24 @@ EncodeTiledFn encode_tiled_fn() {
     return fn;
 }
 
-constexpr int kMapSlots = 8;        // host-side cache of encoded descriptor sets, keyed by (frames ptr, n_frames)
 constexpr int kHostPipeDepth = 3;   // host-buffer pipeline: chunks in flight
 constexpr int kCounterRing = 64;
 constexpr int kMaxStagedPx = 8192;  // largest staged box (pixels, height rounded to 8): 32 KB float tile
-constexpr int kTexSlots = 32;       // host-side cache of texture-object sets, keyed by (frames ptr, n_frames, chunk)
+
+// Host cache of N sets of TMA descriptors or texture objects, keyed by what a set describes (frames pointer, frame count, row
+// pitch, frames per texture object or 0) and refilled round-robin.  No call's frames are at address 0, so the default key marks a
+// slot that holds nothing; a build clears the key first and sets it once the set is complete.
+using FramesKey = std::tuple<const void*, int, int, int>;
+template <class Set, int N>
+struct HostCache {
+    struct Slot { FramesKey key; Set set{}; };
+    Slot slots[N];
+    int next = 0;
+    Set* find(const FramesKey& k) { for (Slot& s : slots) if (s.key == k) return &s.set; return nullptr; }
+    Slot& take() { Slot& s = slots[next]; next = (next + 1) % N; return s; }    // the next slot; the caller releases what it held
+};
+using MapCache = HostCache<TmaMaps*, 8>;                           // 64-byte aligned host memory, reused across keys
+using TexCache = HostCache<std::vector<cudaTextureObject_t>, 32>;   // one object per chunk of frames
 
 }  // namespace
 
@@ -73,18 +87,11 @@ struct mdc_ctx {
     TileDesc* d_tiles = nullptr;
     int* d_counters = nullptr;   // ring of work counters (one per launch in flight)
     unsigned counter_next = 0;
-    // TMA descriptor cache (host memory; descriptors are passed to the kernel by value)
-    TmaMaps* maps[kMapSlots] = {};
-    const void* map_key_ptr[kMapSlots] = {};
-    int map_key_frames[kMapSlots] = {};
-    int map_key_pitch[kMapSlots] = {};
-    int map_next = 0;
-    // texture-gather loader: device limits, self-check verdict, cache of texture-object sets (one object per chunk of frames)
+    MapCache map_cache;                  // TMA descriptor sets (descriptors are passed to the kernel by value)
+    // texture-gather loader: device limits, self-check verdict, cache of texture-object sets
     int tex_max_rows = 0, tex_max_width = 0, tex_pitch_align = 32, tex_base_align = 512;
     bool tex_ok = false;                 // the context-creation self-check found the texture path bit-identical to the staged path
-    struct TexEntry { const void* ptr = nullptr; int n_frames = 0, chunk = 0, pitch = 0; std::vector<cudaTextureObject_t> objs; };
-    TexEntry tex_cache[kTexSlots];
-    int tex_next = 0;
+    TexCache tex_cache;
     // knobs (loader: -1 auto, 0 LDG, 1 TMA, 2 texture gather)
     int use_tma = -1, ctas_per_sm = 0, chunk_frames = 0, tma_stages = 0;
     int tex_tiles_per_cta = 2, tex_prefetch = 0, k1_study = kStudyAll;
@@ -137,6 +144,72 @@ int check_table_domain(const float* rx, const float* ry, int out_w, int out_h, i
     return MDC_OK;
 }
 
+// Input pixels one output tile's taps start from (xlo..xhi-1, ylo..yhi-1; xhi < 0: none), and whether it has black pixels (x < 0)
+struct TileBounds { int xlo = 1 << 30, xhi = -1, ylo = 1 << 30, yhi = -1; bool black = false; };
+
+// Rows of a staged box of pitch `bw` that one pass of the LDG loader covers (rows x words-per-row thread tiling).
+int ldg_row_step(int bw) {
+    int lg = 2;
+    while ((4 << lg) < bw) ++lg;
+    return std::max(1, kThreads >> lg);
+}
+
+// Box width = shared-memory pitch of the staged box of tile t (origin x0, ylo; bh rows, bh8 once rounded to the row granularity).
+// The tap loads of a warp (32 lanes = one output row, 4 byte taps each) are a fixed, calibration-dependent access pattern, so their
+// bank conflicts can be SIMULATED here, per candidate pitch, and traded against the extra bytes TMA has to write for a wider box.
+// Returns the pitch with the fewest shared-memory wavefronts per frame, bw_min when no candidate fits.
+int search_pitch(const mdc_ctx* c, const float* rx, const float* ry, int t, int x0, int ylo, int bh, int bh8, int bw_min) {
+    const int OW = c->out_w, OH = c->out_h;
+    const int tx0 = (t % c->tiles_x) * kTile, ty0 = (t / c->tiles_x) * kTile;
+    int bw = bw_min;
+    long best_cost = -1;
+    for (int pitch = bw_min; pitch <= std::min(bw_min + 112, 256); pitch += 16) {
+        if (pitch * bh8 > kMaxStagedPx) break;
+        const int rs = ldg_row_step(pitch);
+        if ((bh + rs - 1) / rs > kMaxBoxWordsPerThread) break;      // must stay loadable by the LDG loader as well
+        long wavefronts = 0;
+        for (int y = ty0; y < std::min(ty0 + kTile, OH); ++y) {
+            int offs[kTile];
+            int nl = 0;
+            for (int x = tx0; x < std::min(tx0 + kTile, OW); ++x) {
+                const float sx = rx[static_cast<size_t>(y) * OW + x], sy = ry[static_cast<size_t>(y) * OW + x];
+                offs[nl++] = (sx < 0) ? 0 : (static_cast<int>(sy) - ylo) * pitch + (static_cast<int>(sx) - x0);
+            }
+            const int delta[4] = {0, 1, pitch, pitch + 1};
+            for (int d = 0; d < 4; ++d) {
+                int words[32][4], cnt[32];
+                for (int b = 0; b < 32; ++b) cnt[b] = 0;
+                int worst = 1;
+                for (int l = 0; l < nl; ++l) {
+                    const int w = (offs[l] + delta[d]) >> 2, b = w & 31;
+                    bool seen = false;
+                    for (int i = 0; i < cnt[b] && i < 4; ++i) seen |= (words[b][i] == w);
+                    if (!seen) { if (cnt[b] < 4) words[b][cnt[b]] = w; ++cnt[b]; worst = std::max(worst, cnt[b]); }
+                }
+                wavefronts += worst;
+            }
+        }
+        const long cost = wavefronts + pitch * bh8 / 128;   // + wavefronts TMA spends writing the box
+        if (best_cost < 0 || cost < best_cost) { best_cost = cost; bw = pitch; }
+    }
+    return bw;
+}
+
+// MDC_VERBOSE: the plan at row granularity `gran`
+void print_plan(const mdc_ctx* c, int gran) {
+    long staged_bytes = 0; int n_staged = 0, n_direct = 0, n_empty = 0, n_black = 0;
+    for (const TileDesc& t : c->tiles) {
+        const int mode = t.mode_map & 0x0f;
+        if (mode == TILE_STAGED) { staged_bytes += (t.bw_bh & 0xffff) * (t.mode_map >> 16); ++n_staged; }
+        n_direct += mode == TILE_DIRECT;
+        n_empty += mode == TILE_EMPTY;
+        n_black += (t.mode_map & TILE_HAS_BLACK) != 0;
+    }
+    fprintf(stderr, "[mdc] plan: %d tiles (%d staged, %d direct, %d empty, %d with black pixels), %zu TMA box classes at row granularity %d, "
+            "largest box %d B, mean box %ld B\n", static_cast<int>(c->tiles.size()), n_staged, n_direct, n_empty, n_black, c->classes.size(),
+            gran, c->box_px_max, n_staged ? staged_bytes / n_staged : 0);
+}
+
 // Build the tile plan from HOST copies of the remap tables (inside the domain of check_table_domain).
 void build_plan(mdc_ctx* c, const float* rx, const float* ry) {
     const int OW = c->out_w, OH = c->out_h;
@@ -144,114 +217,52 @@ void build_plan(mdc_ctx* c, const float* rx, const float* ry) {
     c->tiles_y = (OH + kTile - 1) / kTile;
     const int n_tiles = c->tiles_x * c->tiles_y;
     c->tiles.assign(n_tiles, TileDesc{0, 0, 0, TILE_EMPTY});
-    // box origins are always 16-byte aligned: whether TMA can be used is decided per call from the ROW PITCH of the frames (a width
-    // that is not a multiple of 16 is fine once the rows are padded, which the host pipeline does during its H2D copy)
-    const bool tma_geom_ok = true;
     const char* e;
     const bool pitch_search = (e = getenv("MDC_PITCH_SEARCH")) ? atoi(e) != 0 : true;
-    // TMA box classes: box heights are rounded up to `gran` rows; coarsen until the shapes fit kMaxClasses
-    for (int gran = 8; gran <= 256; gran *= 2) {
-    c->classes.clear();
-    c->box_px_max = 128;
-    std::map<std::pair<int, int>, int> class_index;
+    std::vector<TileBounds> bounds(n_tiles);
     for (int t = 0; t < n_tiles; ++t) {
         const int tx0 = (t % c->tiles_x) * kTile, ty0 = (t / c->tiles_x) * kTile;
-        int xlo = 1 << 30, xhi = -1, ylo = 1 << 30, yhi = -1;
-        bool black = false;
+        TileBounds& b = bounds[t];
         for (int y = ty0; y < std::min(ty0 + kTile, OH); ++y)
             for (int x = tx0; x < std::min(tx0 + kTile, OW); ++x) {
                 const float sx = rx[static_cast<size_t>(y) * OW + x], sy = ry[static_cast<size_t>(y) * OW + x];
-                if (sx < 0) { black = true; continue; }
+                if (sx < 0) { b.black = true; continue; }
                 const int xi = static_cast<int>(sx), yi = static_cast<int>(sy);
-                xlo = std::min(xlo, xi); xhi = std::max(xhi, xi + 1);
-                ylo = std::min(ylo, yi); yhi = std::max(yhi, yi + 1);
+                b.xlo = std::min(b.xlo, xi); b.xhi = std::max(b.xhi, xi + 1);
+                b.ylo = std::min(b.ylo, yi); b.yhi = std::max(b.yhi, yi + 1);
             }
-        TileDesc td{0, 0, 0, TILE_EMPTY};
-        if (xhi >= 0) {
-            const int x0 = tma_geom_ok ? (xlo & ~15) : (xlo & ~3);   // TMA faults on box origins that are not 16-byte aligned
-            const int bh = yhi - ylo + 1, bh8 = (bh + gran - 1) / gran * gran;
-            // Box width = shared-memory pitch of the staged box.  The tap loads of a warp (32 lanes = one output
-            // row, 4 byte taps each) are a fixed, calibration-dependent access pattern, so their bank conflicts
-            // can be SIMULATED here, per tile and per candidate pitch, and traded against the extra bytes TMA has to
-            // write for a wider box.  Picks the pitch with the fewest shared-memory wavefronts per frame.
-            const int bw_min = ((xhi - x0 + 1) + 15) & ~15;
-            int bw = bw_min;
-            if (pitch_search) {
-                long best_cost = -1;
-                for (int pitch = bw_min; pitch <= std::min(bw_min + 112, 256); pitch += 16) {
-                    if (pitch * bh8 > kMaxStagedPx) break;
-                    {   // must stay loadable by the LDG loader as well (rows x words-per-row thread tiling)
-                        int lgp = 2;
-                        while ((4 << lgp) < pitch) ++lgp;
-                        const int rs = std::max(1, kThreads >> lgp);
-                        if ((bh + rs - 1) / rs > kMaxBoxWordsPerThread) break;
-                    }
-                    long wavefronts = 0;
-                    for (int y = ty0; y < std::min(ty0 + kTile, OH); ++y) {
-                        int offs[kTile];
-                        int nl = 0;
-                        for (int x = tx0; x < std::min(tx0 + kTile, OW); ++x) {
-                            const float sx = rx[static_cast<size_t>(y) * OW + x], sy = ry[static_cast<size_t>(y) * OW + x];
-                            offs[nl++] = (sx < 0) ? 0 : (static_cast<int>(sy) - ylo) * pitch + (static_cast<int>(sx) - x0);
-                        }
-                        const int delta[4] = {0, 1, pitch, pitch + 1};
-                        for (int d = 0; d < 4; ++d) {
-                            int words[32][4], cnt[32];
-                            for (int b = 0; b < 32; ++b) cnt[b] = 0;
-                            int worst = 1;
-                            for (int l = 0; l < nl; ++l) {
-                                const int w = (offs[l] + delta[d]) >> 2, b = w & 31;
-                                bool seen = false;
-                                for (int i = 0; i < cnt[b] && i < 4; ++i) seen |= (words[b][i] == w);
-                                if (!seen) { if (cnt[b] < 4) words[b][cnt[b]] = w; ++cnt[b]; worst = std::max(worst, cnt[b]); }
-                            }
-                            wavefronts += worst;
-                        }
-                    }
-                    const long cost = wavefronts + pitch * bh8 / 128;   // + wavefronts TMA spends writing the box
-                    if (best_cost < 0 || cost < best_cost) { best_cost = cost; bw = pitch; }
+    }
+    // TMA box classes: box heights are rounded up to `gran` rows; coarsen until the shapes fit kMaxClasses
+    for (int gran = 8; gran <= 256; gran *= 2) {
+        c->classes.clear();
+        c->box_px_max = 128;
+        std::map<std::pair<int, int>, int> class_index;
+        for (int t = 0; t < n_tiles; ++t) {
+            const TileBounds& b = bounds[t];
+            TileDesc td{0, 0, 0, TILE_EMPTY};
+            if (b.xhi >= 0) {
+                // box origins are always 16-byte aligned (TMA faults on others): whether TMA can be used is decided per call from the ROW
+                // PITCH of the frames (a width that is not a multiple of 16 is fine once the host pipeline pads the rows in its H2D copy)
+                const int x0 = b.xlo & ~15;
+                const int bh = b.yhi - b.ylo + 1, bh8 = (bh + gran - 1) / gran * gran;
+                const int bw_min = ((b.xhi - x0 + 1) + 15) & ~15;
+                const int bw = pitch_search ? search_pitch(c, rx, ry, t, x0, b.ylo, bh, bh8, bw_min) : bw_min;
+                const int rstep = ldg_row_step(bw);
+                td.x0 = x0; td.y0 = b.ylo; td.bw_bh = bw | (bh << 16);
+                if (bw <= 256 && bh8 <= 256 && bw * bh8 <= kMaxStagedPx && (bh + rstep - 1) / rstep <= kMaxBoxWordsPerThread) {
+                    const auto cls = class_index.emplace(std::make_pair(bw, bh8), static_cast<int>(c->classes.size()));
+                    if (cls.second) c->classes.push_back(cls.first->first);
+                    td.mode_map = TILE_STAGED | (cls.first->second << 8) | (bh8 << 16);
+                    c->box_px_max = std::max(c->box_px_max, bw * bh8);
+                } else {
+                    td.mode_map = TILE_DIRECT;
                 }
             }
-            int lg = 2;
-            while ((4 << lg) < bw) ++lg;
-            const int rstep = std::max(1, kThreads >> lg);
-            const bool staged = bw <= 256 && bh8 <= 256 && bw * bh8 <= kMaxStagedPx &&
-                                (bh + rstep - 1) / rstep <= kMaxBoxWordsPerThread;
-            td.x0 = x0; td.y0 = ylo; td.bw_bh = bw | (bh << 16);
-            if (staged) {
-                int cls = 0;
-                if (tma_geom_ok) {
-                    auto key = std::make_pair(bw, bh8);
-                    auto it = class_index.find(key);
-                    if (it == class_index.end()) {
-                        cls = static_cast<int>(c->classes.size());
-                        class_index[key] = cls;
-                        c->classes.push_back(key);
-                    } else cls = it->second;
-                }
-                td.mode_map = TILE_STAGED | (cls << 8) | (bh8 << 16);
-                c->box_px_max = std::max(c->box_px_max, bw * bh8);
-            } else {
-                td.mode_map = TILE_DIRECT;
-            }
+            if (b.black) td.mode_map |= TILE_HAS_BLACK;
+            c->tiles[t] = td;
         }
-        if (black) td.mode_map |= TILE_HAS_BLACK;
-        c->tiles[t] = td;
-    }
-    if (getenv("MDC_VERBOSE")) {
-        long staged_bytes = 0; int n_staged = 0, n_direct = 0, n_empty = 0, n_black = 0;
-        for (const TileDesc& t : c->tiles) {
-            const int mode = t.mode_map & 0x0f;
-            if (mode == TILE_STAGED) { staged_bytes += (t.bw_bh & 0xffff) * (t.mode_map >> 16); ++n_staged; }
-            n_direct += mode == TILE_DIRECT;
-            n_empty += mode == TILE_EMPTY;
-            n_black += (t.mode_map & TILE_HAS_BLACK) != 0;
-        }
-        fprintf(stderr, "[mdc] plan: %d tiles (%d staged, %d direct, %d empty, %d with black pixels), %zu TMA box classes at row granularity %d, "
-                "largest box %d B, mean box %ld B\n", n_tiles, n_staged, n_direct, n_empty, n_black, c->classes.size(), gran, c->box_px_max,
-                n_staged ? staged_bytes / n_staged : 0);
-    }
-    if (static_cast<int>(c->classes.size()) <= kMaxClasses) break;
+        if (getenv("MDC_VERBOSE")) print_plan(c, gran);
+        if (static_cast<int>(c->classes.size()) <= kMaxClasses) break;
     }
     c->plan_tma_ok = !c->classes.empty() && static_cast<int>(c->classes.size()) <= kMaxClasses && encode_tiled_fn() != nullptr;
 }
@@ -312,10 +323,13 @@ bool tma_pitch_ok(const mdc_ctx* c, const uint8_t* frames, int pitch) {
 }
 
 // ---- texture-gather loader plumbing -------------------------------------------------------------------------------
-// Frames per chunk (= per texture object) for `frames`: as many as the gather height limit allows (at most `want`), such that
-// every chunk starts on a texture-aligned address.  0 = this geometry / pointer cannot use the texture path.
-int tex_chunk_frames(const mdc_ctx* c, const uint8_t* frames, int pitch, int want) {
-    if (pitch % c->tex_pitch_align != 0 || c->in_w > c->tex_max_width || c->in_h < 2) return 0;
+bool tex_pitch_ok(const mdc_ctx* c, int pitch) { return pitch % c->tex_pitch_align == 0; }
+
+// Frames per chunk (= per texture object) for `frames`: as many as the gather height limit allows (at most the schedule chunk of
+// MDC_CHUNK_FRAMES), such that every chunk starts on a texture-aligned address.  0 = this geometry / pointer cannot use the texture path.
+int tex_chunk_frames(const mdc_ctx* c, const uint8_t* frames, int pitch) {
+    const int want = c->chunk_frames > 0 ? c->chunk_frames : 48;
+    if (!tex_pitch_ok(c, pitch) || c->in_w > c->tex_max_width || c->in_h < 2) return 0;
     if (reinterpret_cast<uintptr_t>(frames) % static_cast<uintptr_t>(c->tex_base_align) != 0) return 0;
     const long long frame_bytes = static_cast<long long>(pitch) * c->in_h;
     for (int n = std::min(want, c->tex_max_rows / c->in_h); n >= 1; --n)
@@ -323,85 +337,76 @@ int tex_chunk_frames(const mdc_ctx* c, const uint8_t* frames, int pitch, int wan
     return 0;
 }
 
-void tex_entry_release(mdc_ctx::TexEntry& e) {
-    for (cudaTextureObject_t t : e.objs) cudaDestroyTextureObject(t);
-    e.objs.clear();
-    e.ptr = nullptr;
+void tex_release(TexCache::Slot& s) {
+    for (cudaTextureObject_t t : s.set) cudaDestroyTextureObject(t);
+    s.set.clear();
+    s.key = FramesKey();
 }
 
 // texture objects for `frames` ([n_frames][H][W] u8) cut into chunks of `chunk` frames; cached on the host
 int get_textures(mdc_ctx* c, const uint8_t* frames, int pitch, int n_frames, int chunk, const std::vector<cudaTextureObject_t>** out) {
-    for (int s = 0; s < kTexSlots; ++s) {
-        mdc_ctx::TexEntry& e = c->tex_cache[s];
-        if (e.ptr == frames && e.n_frames == n_frames && e.chunk == chunk && e.pitch == pitch) { *out = &e.objs; return MDC_OK; }
-    }
-    mdc_ctx::TexEntry& e = c->tex_cache[c->tex_next];
-    c->tex_next = (c->tex_next + 1) % kTexSlots;
-    if (e.ptr) {                       // evicting: a launch that still reads these objects may be in flight on any stream
+    const FramesKey key{frames, n_frames, pitch, chunk};
+    if ((*out = c->tex_cache.find(key))) return MDC_OK;
+    TexCache::Slot& s = c->tex_cache.take();
+    if (!s.set.empty()) {              // evicting: a launch that still reads these objects may be in flight on any stream
         CU_CHECK(cudaDeviceSynchronize());
-        tex_entry_release(e);
+        tex_release(s);
     }
     const int n_chunks = (n_frames + chunk - 1) / chunk;
     const size_t frame_bytes = static_cast<size_t>(pitch) * c->in_h;
     for (int k = 0; k < n_chunks; ++k) {
         const int nf = std::min(chunk, n_frames - k * chunk);
-        cudaResourceDesc rd;
-        memset(&rd, 0, sizeof rd);
+        cudaResourceDesc rd = {};
         rd.resType = cudaResourceTypePitch2D;
         rd.res.pitch2D.devPtr = const_cast<uint8_t*>(frames) + static_cast<size_t>(k) * chunk * frame_bytes;
         rd.res.pitch2D.desc = cudaCreateChannelDesc(8, 0, 0, 0, cudaChannelFormatKindUnsigned);
         rd.res.pitch2D.width = static_cast<size_t>(c->in_w);
         rd.res.pitch2D.height = static_cast<size_t>(c->in_h) * nf;
         rd.res.pitch2D.pitchInBytes = static_cast<size_t>(pitch);
-        cudaTextureDesc td;
-        memset(&td, 0, sizeof td);
+        cudaTextureDesc td = {};      // unnormalised coordinates
         td.addressMode[0] = td.addressMode[1] = td.addressMode[2] = cudaAddressModeClamp;
         td.filterMode = cudaFilterModePoint;
         td.readMode = cudaReadModeElementType;
-        td.normalizedCoords = 0;
         cudaTextureObject_t t = 0;
         cudaError_t err = cudaCreateTextureObject(&t, &rd, &td, nullptr);
         if (err != cudaSuccess) {
             mdc_set_error("cudaCreateTextureObject failed: %s (chunk %d, %d x %d rows)", cudaGetErrorString(err), k, c->in_w, c->in_h * nf);
-            tex_entry_release(e);
+            tex_release(s);
             return MDC_ERR_CUDA;
         }
-        e.objs.push_back(t);
+        s.set.push_back(t);
     }
-    e.ptr = frames; e.n_frames = n_frames; e.chunk = chunk; e.pitch = pitch;
-    *out = &e.objs;
+    s.key = key;
+    *out = &s.set;
     return MDC_OK;
 }
 
 // descriptors for `frames` ([n_frames][H][W] u8): one per box class; encoded sets are cached on the host
 int get_tensor_maps(mdc_ctx* c, const uint8_t* frames, int pitch, int n_frames, const TmaMaps** out) {
-    for (int s = 0; s < kMapSlots; ++s)
-        if (c->maps[s] && c->map_key_ptr[s] == frames && c->map_key_frames[s] == n_frames && c->map_key_pitch[s] == pitch) { *out = c->maps[s]; return MDC_OK; }
+    const FramesKey key{frames, n_frames, pitch, 0};
+    if (TmaMaps* const* hit = c->map_cache.find(key)) { *out = *hit; return MDC_OK; }
     EncodeTiledFn enc = encode_tiled_fn();
     if (!enc) { mdc_set_error("cuTensorMapEncodeTiled unavailable"); return MDC_ERR_CUDA; }
-    const int slot = c->map_next;
-    c->map_next = (c->map_next + 1) % kMapSlots;
-    if (!c->maps[slot]) {
+    MapCache::Slot& s = c->map_cache.take();
+    if (!s.set) {
         void* mem = nullptr;
         if (posix_memalign(&mem, 64, sizeof(TmaMaps)) != 0) { mdc_set_error("out of memory"); return MDC_ERR_CUDA; }
         memset(mem, 0, sizeof(TmaMaps));
-        c->maps[slot] = static_cast<TmaMaps*>(mem);
+        s.set = static_cast<TmaMaps*>(mem);
     }
-    c->map_key_ptr[slot] = nullptr;
+    s.key = FramesKey();
     for (size_t i = 0; i < c->classes.size(); ++i) {
         const cuuint64_t dims[3] = {static_cast<cuuint64_t>(c->in_w), static_cast<cuuint64_t>(c->in_h), static_cast<cuuint64_t>(n_frames)};
         const cuuint64_t strides[2] = {static_cast<cuuint64_t>(pitch), static_cast<cuuint64_t>(pitch) * c->in_h};
         const cuuint32_t box[3] = {static_cast<cuuint32_t>(c->classes[i].first), static_cast<cuuint32_t>(c->classes[i].second), 1u};
         const cuuint32_t estr[3] = {1u, 1u, 1u};
-        CUresult r = enc(&c->maps[slot]->m[i], CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<uint8_t*>(frames), dims, strides, box, estr,
+        CUresult r = enc(&s.set->m[i], CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<uint8_t*>(frames), dims, strides, box, estr,
                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) { mdc_set_error("cuTensorMapEncodeTiled failed (%d) for box %u x %u", (int)r, box[0], box[1]); return MDC_ERR_CUDA; }
     }
-    c->map_key_ptr[slot] = frames;
-    c->map_key_frames[slot] = n_frames;
-    c->map_key_pitch[slot] = pitch;
-    *out = c->maps[slot];
+    s.key = key;
+    *out = s.set;
     return MDC_OK;
 }
 
@@ -463,7 +468,7 @@ void k2_sources(bool rectify, int levels, bool need[MDC_MAX_PYR_LEVELS]) {
 }
 
 // levels beyond the fused epilogue: stand-alone K2 chain, two levels per launch where possible
-int run_deep_levels(mdc_ctx* c, int n_frames, const Outs& o, int in_kernel, int levels, cudaStream_t stream) {
+int run_deep_levels(mdc_ctx* c, int n_frames, const Outs& o, int in_kernel, int levels, cudaStream_t stream, long long& launches) {
     for (int l = in_kernel; l < levels;) {
         const int sw = c->out_w >> (l - 1), sh = c->out_h >> (l - 1);
         if (l + 1 < levels) {
@@ -473,48 +478,50 @@ int run_deep_levels(mdc_ctx* c, int n_frames, const Outs& o, int in_kernel, int 
             CU_CHECK(launch_pyr_down(o.src(l - 1), sw, sh, o.lv[l], o.type, nullptr, n_frames, stream));
             l += 1;
         }
-        c->launches++;
+        launches++;
     }
     return MDC_OK;
 }
 
-// K1 through the texture-gather loader.  One launch covers up to kMaxTex chunks (= texture objects).
-int run_fused_tex(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frames, int chunk, UnmapFlags u, const Outs& outs, int levels,
-                  cudaStream_t stream) {
+// The FusedParams fields of every K1 launch, for n_frames frames from `frames` into levels 0..in_kernel-1 of `outs`.  Everything
+// else starts zeroed (unused_, lw / lh past in_kernel, the loader's own fields), so equal calls pass equal parameter bytes.
+void fused_params(FusedParams& p, const mdc_ctx* c, const uint8_t* frames, int pitch, int n_frames, UnmapFlags u, const Outs& outs,
+                  int in_kernel) {
+    memset(&p, 0, sizeof p);
+    p.frames = frames; p.n_frames = n_frames;
+    p.in_w = c->in_w; p.in_h = c->in_h; p.out_w = c->out_w; p.out_h = c->out_h; p.in_pitch = pitch;
+    p.remap_x = c->d_rx; p.remap_y = c->d_ry; p.vinv = c->d_vinv; p.ginv = c->d_ginv;
+    p.tiles = c->d_tiles;
+    p.tiles_x = c->tiles_x; p.n_tiles = static_cast<int>(c->tiles.size());
+    p.levels = in_kernel;
+    for (int l = 0; l < in_kernel; ++l) { p.out[l] = outs.lv[l]; p.lw[l] = c->out_w >> l; p.lh[l] = c->out_h >> l; }
+    p.level2_f32 = outs.f32[2];
+    p.lut_gamma = u.gamma; p.use_vig = u.vig; p.kill = u.kill;
+    p.carveout = c->carveout;
+}
+
+// K1 through the texture-gather loader, levels 0..in_kernel-1.  One launch covers up to kMaxTex chunks (= texture objects).
+int run_fused_tex(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frames, int chunk, UnmapFlags u, const Outs& outs, int in_kernel,
+                  int study, cudaStream_t stream, long long& launches) {
     const std::vector<cudaTextureObject_t>* objs = nullptr;
     int rc = get_textures(c, d_frames, pitch, n_frames, chunk, &objs);
     if (rc != MDC_OK) return rc;
-    const int in_kernel = std::min(levels, kInKernelLevels);
     const int n_chunks = static_cast<int>(objs->size());
     const int min_ctas = c->ctas_per_sm > 0 ? std::min(std::max(c->ctas_per_sm, 2), 4) : 3;
     for (int c0 = 0; c0 < n_chunks; c0 += kMaxTex) {
         const int nc = std::min(kMaxTex, n_chunks - c0);
         const int f0 = c0 * chunk, nf = std::min(n_frames - f0, nc * chunk);
         FusedParams p;
-        memset(&p, 0, sizeof p);
-        p.frames = d_frames + static_cast<size_t>(f0) * pitch * c->in_h; p.n_frames = nf;
-        p.in_w = c->in_w; p.in_h = c->in_h; p.out_w = c->out_w; p.out_h = c->out_h; p.in_pitch = pitch;
-        p.remap_x = c->d_rx; p.remap_y = c->d_ry; p.vinv = c->d_vinv; p.ginv = c->d_ginv;
-        p.tiles = c->d_tiles; p.work_counter = nullptr;
-        p.tiles_x = c->tiles_x; p.n_tiles = static_cast<int>(c->tiles.size());
-        p.levels = in_kernel;
-        const Outs o = outs.from(static_cast<size_t>(f0));
-        for (int l = 0; l < in_kernel; ++l) {
-            p.lw[l] = c->out_w >> l; p.lh[l] = c->out_h >> l;
-            p.out[l] = o.lv[l];
-        }
-        p.level2_f32 = o.f32[2];
-        p.lut_gamma = u.gamma; p.use_vig = u.vig; p.kill = u.kill;
+        fused_params(p, c, d_frames + static_cast<size_t>(f0) * pitch * c->in_h, pitch, nf, u, outs.from(static_cast<size_t>(f0)), in_kernel);
         p.chunk_frames = chunk;
         p.tiles_per_cta = c->tex_tiles_per_cta;
-        p.carveout = c->carveout;
         TexSet texs;
         memset(&texs, 0, sizeof texs);
         for (int k = 0; k < nc; ++k) texs.tex[k] = (*objs)[c0 + k];
-        CU_CHECK(launch_fused_tex(p, texs, nc, min_ctas, c->tex_prefetch != 0, c->k1_study, outs.type, stream));
-        c->launches++;
+        CU_CHECK(launch_fused_tex(p, texs, nc, min_ctas, c->tex_prefetch != 0, study, outs.type, stream));
+        launches++;
     }
-    return run_deep_levels(c, n_frames, outs, in_kernel, levels, stream);
+    return MDC_OK;
 }
 
 // What "auto" resolves to (order measured on H100 at 1280x1024: TMA ahead of hybrid and texture gather, DESIGN.md §7); a loader that turns out unusable for a particular
@@ -527,29 +534,16 @@ int auto_loader(const mdc_ctx* c, const uint8_t* frames, int pitch) {
     return 0;
 }
 
-// K1 through the staged loaders (TMA ring or LDG double buffer), levels 0..in_kernel-1 only.  cap_per_sm > 0 bounds the persistent
-// grid (hybrid mode leaves room for the texture kernel's CTAs on every SM).
-int run_fused_staged(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frames, UnmapFlags u, const Outs& outs, int in_kernel,
-                     cudaStream_t stream, int loader, int cap_per_sm) {
+// K1 through a staged loader, the TMA ring (tma) or the LDG double buffer, levels 0..in_kernel-1.  cap_per_sm > 0 bounds the
+// persistent grid (hybrid mode leaves room for the texture kernel's CTAs on every SM).
+int run_fused_staged(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frames, UnmapFlags u, const Outs& outs, int in_kernel, bool tma,
+                     int cap_per_sm, int study, cudaStream_t stream, long long& launches) {
     FusedParams p;
-    memset(&p, 0, sizeof p);
-    p.frames = d_frames; p.n_frames = n_frames;
-    p.in_w = c->in_w; p.in_h = c->in_h; p.out_w = c->out_w; p.out_h = c->out_h; p.in_pitch = pitch;
-    p.remap_x = c->d_rx; p.remap_y = c->d_ry; p.vinv = c->d_vinv; p.ginv = c->d_ginv;
-    p.tiles = c->d_tiles;
+    fused_params(p, c, d_frames, pitch, n_frames, u, outs, in_kernel);
     p.work_counter = c->d_counters + (c->counter_next++ % kCounterRing);
     CU_CHECK(cudaMemsetAsync(p.work_counter, 0, sizeof(int), stream));
-    p.tiles_x = c->tiles_x; p.n_tiles = static_cast<int>(c->tiles.size());
-    p.levels = in_kernel;
-    for (int l = 0; l < in_kernel; ++l) { p.out[l] = outs.lv[l]; p.lw[l] = c->out_w >> l; p.lh[l] = c->out_h >> l; }
-    for (int l = in_kernel; l < MDC_MAX_PYR_LEVELS; ++l) { p.lw[l] = p.lh[l] = 0; }
-    p.level2_f32 = outs.f32[2];
-    p.lut_gamma = u.gamma; p.use_vig = u.vig; p.kill = u.kill;
     p.box_px_max = c->box_px_max;
-    p.carveout = c->carveout;
     p.chunk_frames = c->chunk_frames > 0 ? c->chunk_frames : 48;
-    bool tma = loader != 0 && tma_pitch_ok(c, d_frames, pitch);
-    if (loader == 1 && !tma) { mdc_set_error("TMA loader requested but unusable for this geometry/pointer"); return MDC_ERR_UNSUPPORTED; }
     const TmaMaps* maps = nullptr;
     if (tma) {
         int rc = get_tensor_maps(c, d_frames, pitch, n_frames, &maps);
@@ -566,10 +560,10 @@ int run_fused_staged(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frame
     if (cap_per_sm > 0) per_sm = std::min(per_sm, cap_per_sm);
     const long long items = static_cast<long long>(p.n_tiles) * ((n_frames + p.chunk_frames - 1) / p.chunk_frames);
     int grid = static_cast<int>(std::min<long long>(static_cast<long long>(per_sm) * c->sm_count, std::max<long long>(items, 1)));
-    if (c->k1_study != kStudyAll && tma && u.vig && in_kernel == 1 && min_ctas == 3 && outs.type == MDC_OUT_F32)
-        CU_CHECK(launch_fused_study(p, maps, grid, c->k1_study, stream));
+    if (study != kStudyAll && tma && u.vig && in_kernel == 1 && min_ctas == 3 && outs.type == MDC_OUT_F32)
+        CU_CHECK(launch_fused_study(p, maps, grid, study, stream));
     else CU_CHECK(launch_fused(p, maps, grid, min_ctas, outs.type, stream));
-    c->launches++;
+    launches++;
     return MDC_OK;
 }
 
@@ -577,59 +571,70 @@ int run_fused_staged(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frame
 // stores on the LSU / shared-memory pipe) with a reduced persistent grid, and the texture-gather kernel (taps on the TEX pipe) in
 // the register / shared-memory space that is left.  The idea is that the two pipes add up; on H100 it is
 // slower than the TMA kernel alone (DESIGN.md §7), so `auto` picks it only on request (MDC_AUTO_HYBRID).
-// The leading whole chunks go to the texture kernel, the rest to the staged kernel; fork/join with events around an auxiliary stream.
-int run_fused_hybrid(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frames, int chunk, UnmapFlags u, const Outs& outs, int levels,
-                     cudaStream_t stream) {
-    const int in_kernel = std::min(levels, kInKernelLevels);
-    const int n_chunks = (n_frames + chunk - 1) / chunk;
-    int tex_chunks = static_cast<int>((static_cast<long long>(n_chunks) * c->hyb_tex_pct + 50) / 100);
-    tex_chunks = std::max(0, std::min(tex_chunks, n_chunks));
-    const int n_tex = std::min(n_frames, tex_chunks * chunk), n_stg = n_frames - n_tex;
-    if (n_tex == 0 || n_stg == 0 || !tma_pitch_ok(c, d_frames, pitch)) {
-        if (n_stg == 0) return run_fused_tex(c, d_frames, pitch, n_frames, chunk, u, outs, levels, stream);
-        int rc = run_fused_staged(c, d_frames, pitch, n_frames, u, outs, in_kernel, stream, -1, 0);
-        return rc != MDC_OK ? rc : run_deep_levels(c, n_frames, outs, in_kernel, levels, stream);
-    }
+// The leading n_tex frames go to the texture kernel, the rest to the TMA kernel; fork/join with events around an auxiliary stream.
+int run_fused_hybrid(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frames, int n_tex, int chunk, UnmapFlags u, const Outs& outs,
+                     int in_kernel, int study, cudaStream_t stream, long long& launches) {
     if (!c->aux_stream) {
         CU_CHECK(cudaStreamCreateWithFlags(&c->aux_stream, cudaStreamNonBlocking));
         CU_CHECK(cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming));
         CU_CHECK(cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming));
     }
-    const Outs stg_out = outs.from(static_cast<size_t>(n_tex));
     CU_CHECK(cudaEventRecord(c->ev_fork, stream));
     CU_CHECK(cudaStreamWaitEvent(c->aux_stream, c->ev_fork, 0));
     // staged kernel first: its persistent CTAs take their slots on every SM, the texture kernel's short CTAs fill what is left
-    int rc = run_fused_staged(c, d_frames + static_cast<size_t>(n_tex) * pitch * c->in_h, pitch, n_stg, u, stg_out, in_kernel, stream, 1, c->hyb_stg_ctas);
+    int rc = run_fused_staged(c, d_frames + static_cast<size_t>(n_tex) * pitch * c->in_h, pitch, n_frames - n_tex, u,
+                              outs.from(static_cast<size_t>(n_tex)), in_kernel, true, c->hyb_stg_ctas, study, stream, launches);
     if (rc != MDC_OK) return rc;
-    rc = run_fused_tex(c, d_frames, pitch, n_tex, chunk, u, outs, in_kernel, c->aux_stream);
+    rc = run_fused_tex(c, d_frames, pitch, n_tex, chunk, u, outs, in_kernel, study, c->aux_stream, launches);
     if (rc != MDC_OK) return rc;
     CU_CHECK(cudaEventRecord(c->ev_join, c->aux_stream));
     CU_CHECK(cudaStreamWaitEvent(stream, c->ev_join, 0));
-    return run_deep_levels(c, n_frames, outs, in_kernel, levels, stream);
+    return MDC_OK;
 }
 
-// loader: -1 = the context's setting (auto: see mdc_ctx_configure); pitch = bytes between input rows (0 = tightly packed)
-int run_fused(mdc_ctx* c, const uint8_t* d_frames, int n_frames, UnmapFlags u, const Outs& outs, int levels,
-              cudaStream_t stream, int loader = -1, int pitch = 0) {
-    if (pitch <= 0) pitch = c->in_w;
+// What one K1 call runs: `loader` (MDC_LOADER_*), for the texture and hybrid loaders the frames per texture object (`chunk`), and
+// for the hybrid loader the leading frames the texture kernel takes (`n_tex`); or, where `refusal` is set, why the call cannot run.
+struct K1Route { int loader, chunk, n_tex; const char* refusal; };
+
+// The loader rule.  `loader` is the call's own request (only the self-check makes one), or -1 for the context's setting
+// (mdc_ctx_configure / MDC_USE_TMA; -1 = auto_loader).  A texture or hybrid loader set on the context refuses a call it cannot
+// serve; "auto" and the self-check fall back to TMA instead, or to LDG where TMA cannot describe the frames either.
+K1Route route_k1(const mdc_ctx* c, const uint8_t* frames, int pitch, int n_frames, int loader) {
+    const bool forced_tex = loader < 0 && c->use_tma >= 2;
     if (loader < 0) loader = c->use_tma;
-    if (loader < 0) loader = auto_loader(c, d_frames, pitch);
-    if (loader == 2 || loader == 3) {
-        if (c->use_tma >= 2 && !c->tex_ok) {
-            mdc_set_error("texture-gather loader requested, but its self-check did not pass on this device / geometry");
-            return MDC_ERR_UNSUPPORTED;
-        }
-        const int chunk = tex_chunk_frames(c, d_frames, pitch, c->chunk_frames > 0 ? c->chunk_frames : 48);
-        if (chunk > 0) {
-            if (loader == 3) return run_fused_hybrid(c, d_frames, pitch, n_frames, chunk, u, outs, levels, stream);
-            return run_fused_tex(c, d_frames, pitch, n_frames, chunk, u, outs, levels, stream);
-        }
-        if (c->use_tma >= 2) { mdc_set_error("texture-gather loader requested but unusable for this geometry/pointer"); return MDC_ERR_UNSUPPORTED; }
-        loader = tma_pitch_ok(c, d_frames, pitch) ? 1 : 0;      // auto: this pointer / batch cannot go through textures
-    }
+    if (loader < 0) loader = auto_loader(c, frames, pitch);
+    const bool tma = tma_pitch_ok(c, frames, pitch);
+    const K1Route staged{tma ? MDC_LOADER_TMA : MDC_LOADER_LDG, 0, 0, nullptr};
+    const auto refuse = [](const char* why) { return K1Route{MDC_LOADER_LDG, 0, 0, why}; };
+    if (loader == MDC_LOADER_LDG) return K1Route{MDC_LOADER_LDG, 0, 0, nullptr};
+    if (loader == MDC_LOADER_TMA && !tma) return refuse("TMA loader requested but unusable for this geometry/pointer");
+    if (loader != MDC_LOADER_TEX && loader != MDC_LOADER_HYBRID) return staged;
+    if (forced_tex && !c->tex_ok) return refuse("texture-gather loader requested, but its self-check did not pass on this device / geometry");
+    const int chunk = tex_chunk_frames(c, frames, pitch);
+    if (chunk == 0) return forced_tex ? refuse("texture-gather loader requested but unusable for this geometry/pointer") : staged;
+    if (loader == MDC_LOADER_TEX) return K1Route{MDC_LOADER_TEX, chunk, 0, nullptr};
+    // hybrid: the texture kernel takes the leading hyb_tex_pct percent of the chunks
+    const int n_chunks = (n_frames + chunk - 1) / chunk;
+    const int tex_chunks = std::max(0, std::min(static_cast<int>((static_cast<long long>(n_chunks) * c->hyb_tex_pct + 50) / 100), n_chunks));
+    const int n_tex = std::min(n_frames, tex_chunks * chunk);
+    if (n_tex == n_frames) return K1Route{MDC_LOADER_TEX, chunk, 0, nullptr};
+    if (n_tex == 0 || !tma) return staged;
+    return K1Route{MDC_LOADER_HYBRID, chunk, n_tex, nullptr};
+}
+
+// K1 and the K2 chain behind it, through the loader route_k1 picks for `loader` (-1 = the context's setting), with the floor-study
+// bits `study`; every launch is counted in `launches`.  pitch = bytes between input rows (0 = tightly packed).
+int run_fused(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frames, UnmapFlags u, const Outs& outs, int levels, cudaStream_t stream,
+              int loader, int study, long long& launches) {
+    if (pitch <= 0) pitch = c->in_w;
+    const K1Route r = route_k1(c, d_frames, pitch, n_frames, loader);
+    if (r.refusal) { mdc_set_error("%s", r.refusal); return MDC_ERR_UNSUPPORTED; }
     const int in_kernel = std::min(levels, kInKernelLevels);
-    int rc = run_fused_staged(c, d_frames, pitch, n_frames, u, outs, in_kernel, stream, loader, 0);
-    return rc != MDC_OK ? rc : run_deep_levels(c, n_frames, outs, in_kernel, levels, stream);
+    const int rc =
+        r.loader == MDC_LOADER_TEX    ? run_fused_tex(c, d_frames, pitch, n_frames, r.chunk, u, outs, in_kernel, study, stream, launches)
+        : r.loader == MDC_LOADER_HYBRID ? run_fused_hybrid(c, d_frames, pitch, n_frames, r.n_tex, r.chunk, u, outs, in_kernel, study, stream, launches)
+        : run_fused_staged(c, d_frames, pitch, n_frames, u, outs, in_kernel, r.loader == MDC_LOADER_TMA, 0, study, stream, launches);
+    return rc != MDC_OK ? rc : run_deep_levels(c, n_frames, outs, in_kernel, levels, stream, launches);
 }
 
 // Self-check of the texture-gather loader, run once per context: K1 over three synthetic frames (all byte values, saturated
@@ -654,7 +659,7 @@ void tex_selfcheck(mdc_ctx* c) {
     if (cudaMalloc(&raw, static_cast<size_t>(nf) * pitch * c->in_h + 1024) != cudaSuccess || cudaMalloc(&out_a, nf * n_out * 4) != cudaSuccess ||
         cudaMalloc(&out_b, nf * n_out * 4) != cudaSuccess || cudaMalloc(&d_bad, 8) != cudaSuccess) { cleanup(); return; }
     uint8_t* frames = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw) + 511) & ~static_cast<uintptr_t>(511));
-    const int chunk = tex_chunk_frames(c, frames, pitch, c->chunk_frames > 0 ? c->chunk_frames : 48);
+    const int chunk = tex_chunk_frames(c, frames, pitch);
     if (chunk < 1) { if (verbose) fprintf(stderr, "[mdc] texture-gather loader: geometry not describable (pitch %d, limit %d rows)\n", c->in_w, c->tex_max_rows); cleanup(); return; }
     std::vector<uint8_t> h(nf * n_in);
     uint32_t lcg = 12345u;
@@ -665,22 +670,17 @@ void tex_selfcheck(mdc_ctx* c) {
               cudaMemset(out_a, 0xff, nf * n_out * 4) == cudaSuccess && cudaMemset(out_b, 0, nf * n_out * 4) == cudaSuccess &&
               cudaMemset(d_bad, 0, 8) == cudaSuccess;
     const UnmapFlags u{c->have_gamma, c->have_gamma && c->have_vig, true};
-    float* la[1] = {out_a};
-    float* lb[1] = {out_b};
-    const long long launches0 = c->launches;
-    const int study0 = c->k1_study, use_tma0 = c->use_tma;
-    c->k1_study = kStudyAll;             // the floor-study variants compute garbage by design
-    c->use_tma = -1;                     // MDC_USE_TMA=2/3 would refuse the texture loader while tex_ok is still false
-    ok = ok && run_fused(c, frames, nf, u, f32_outs(la, 1, c), 1, c->stream, 2, pitch) == MDC_OK;
+    // its own loader requests (MDC_USE_TMA=2/3 would refuse the texture loader while tex_ok is still false), all study bits (the
+    // floor-study variants compute garbage by design), and its own launch count (the context's counts the caller's launches only)
+    long long launches = 0;
+    ok = ok && run_fused(c, frames, pitch, nf, u, f32_outs(&out_a, 1, c), 1, c->stream, MDC_LOADER_TEX, kStudyAll, launches) == MDC_OK;
     const bool tma_ref = tma_pitch_ok(c, frames, pitch);
-    ok = ok && run_fused(c, frames, nf, u, f32_outs(lb, 1, c), 1, c->stream, tma_ref ? 1 : 0, pitch) == MDC_OK;
-    c->k1_study = study0;
-    c->use_tma = use_tma0;
+    ok = ok && run_fused(c, frames, pitch, nf, u, f32_outs(&out_b, 1, c), 1, c->stream, tma_ref ? MDC_LOADER_TMA : MDC_LOADER_LDG, kStudyAll,
+                         launches) == MDC_OK;
     ok = ok && launch_count_mismatch(out_a, out_b, nf * n_out, d_bad, c->stream) == cudaSuccess;
     unsigned long long bad = ~0ull;
     ok = ok && cudaMemcpyAsync(&bad, d_bad, 8, cudaMemcpyDeviceToHost, c->stream) == cudaSuccess && cudaStreamSynchronize(c->stream) == cudaSuccess;
-    c->launches = launches0;             // bookkeeping counts the caller's launches only
-    for (auto& t : c->tex_cache) if (t.ptr == frames) tex_entry_release(t);
+    for (auto& s : c->tex_cache.slots) if (std::get<0>(s.key) == frames) tex_release(s);
     c->tex_ok = ok && bad == 0;
     if (verbose || (ok && bad != 0))
         fprintf(stderr, "[mdc] texture-gather loader self-check: %s (%llu of %zu output words differ from the %s loader; chunk = %d frames)\n",
@@ -792,9 +792,9 @@ extern "C" void mdc_ctx_destroy(mdc_ctx* c) {
     if (c->stream) cudaStreamSynchronize(c->stream);
     if (c->owns_tables) { cudaFree(c->d_rx); cudaFree(c->d_ry); cudaFree(c->d_ginv); cudaFree(c->d_vinv); }
     cudaFree(c->d_tiles); cudaFree(c->d_counters); cudaFree(c->d_rc);
-    for (int s = 0; s < kMapSlots; ++s) free(c->maps[s]);
+    for (auto& s : c->map_cache.slots) free(s.set);
     cudaDeviceSynchronize();
-    for (auto& t : c->tex_cache) tex_entry_release(t);
+    for (auto& s : c->tex_cache.slots) tex_release(s);
     if (c->aux_stream) { cudaStreamDestroy(c->aux_stream); cudaEventDestroy(c->ev_fork); cudaEventDestroy(c->ev_join); }
     for (int s = 0; s < kHostPipeDepth; ++s) {
         if (c->pipe_stream[s]) { cudaStreamSynchronize(c->pipe_stream[s]); cudaStreamDestroy(c->pipe_stream[s]); }
@@ -846,8 +846,8 @@ extern "C" int mdc_ctx_loader_usable_pitched(const mdc_ctx* c, int loader, size_
     switch (loader) {
         case MDC_LOADER_LDG: return 1;
         case MDC_LOADER_TMA: return tma_pitch_ok(c, nullptr, pitch) ? 1 : 0;
-        case MDC_LOADER_TEX: return (c->tex_ok && pitch % c->tex_pitch_align == 0) ? 1 : 0;
-        case MDC_LOADER_HYBRID: return (c->tex_ok && pitch % c->tex_pitch_align == 0 && tma_pitch_ok(c, nullptr, pitch)) ? 1 : 0;
+        case MDC_LOADER_TEX: return (c->tex_ok && tex_pitch_ok(c, pitch)) ? 1 : 0;
+        case MDC_LOADER_HYBRID: return (c->tex_ok && tex_pitch_ok(c, pitch) && tma_pitch_ok(c, nullptr, pitch)) ? 1 : 0;
         default: return 0;
     }
 }
@@ -893,8 +893,7 @@ extern "C" int mdc_undistort_u8(mdc_ctx* c, const uint8_t* d_in, float* d_out, i
     if (n_frames == 0) return MDC_OK;
     CU_CHECK(cudaSetDevice(c->device));
     cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
-    float* lv[1] = {d_out};
-    rc = run_fused(c, d_in, n_frames, UnmapFlags{false, false, false}, f32_outs(lv, 1, c), 1, s);
+    rc = run_fused(c, d_in, 0, n_frames, UnmapFlags{false, false, false}, f32_outs(&d_out, 1, c), 1, s, -1, c->k1_study, c->launches);
     if (rc != MDC_OK) return rc;
     return finish(c, stream, s);
 }
@@ -1025,7 +1024,7 @@ static int prepare_batch_impl(mdc_ctx* c, const uint8_t* d_frames, int pitch, in
     UnmapFlags u{false, false, false};
     if (photometric) u = sanitise(c, flags);
     if (rectify) {
-        rc = run_fused(c, d_frames, n_frames, u, o, levels, s, -1, pitch);
+        rc = run_fused(c, d_frames, pitch, n_frames, u, o, levels, s, -1, c->k1_study, c->launches);
     } else if (pitch > 0 && pitch != c->in_w) {
         mdc_set_error("padded rows are supported in rectifying mode only");
         rc = MDC_ERR_UNSUPPORTED;

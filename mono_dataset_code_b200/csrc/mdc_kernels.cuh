@@ -28,7 +28,7 @@ enum TileMode : int { TILE_EMPTY = 0, TILE_STAGED = 1, TILE_DIRECT = 2, TILE_HAS
 
 // One output tile of the rectification plan (built once per context from the remap tables).
 struct alignas(16) TileDesc {
-    int x0, y0;        // origin of the input bounding box (x0 is a multiple of 16 when TMA can be used, else of 4)
+    int x0, y0;        // origin of the input bounding box (x0 is a multiple of 16: TMA box origins must be 16-byte aligned)
     int bw_bh;         // box width (multiple of 16, also the smem pitch) | box height << 16
     int mode_map;      // TileMode (low nibble) | TILE_HAS_BLACK | (tensor-map class index << 8) | (TMA box height << 16)
 };
