@@ -128,6 +128,10 @@ const float* mdc_photo_vignette_map_inv(const mdc_photo* p); /* vignetteMapInv (
  * Device context — tables uploaded once, resident in HBM; tile plan + TMA descriptors.
  * One context per GPU (one process per GPU).  fov and/or photo may be NULL/invalid:
  * operations needing the missing half then fail with MDC_ERR_INVALID_OBJECT.
+ * Concurrency: one context may be used from several streams, by one host thread at a time
+ * (its host caches and pipeline buffers are not locked).  Different contexts, on the same
+ * device or not, may be used from different host threads at once, and may be created at
+ * the same time.  The responseCalib calls keep their own rule (see below).
  * ===================================================================================== */
 int mdc_ctx_create(int device, const mdc_fov* fov, const mdc_photo* photo, mdc_ctx** out);
 /* Multi-GPU init: rank 0 builds the host models, broadcasts the four tables over NCCL

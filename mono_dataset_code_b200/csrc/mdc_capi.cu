@@ -36,17 +36,15 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
+// Looked up once per process; a function-local static is initialised once even when several threads create contexts at once.
 EncodeTiledFn encode_tiled_fn() {
-    static EncodeTiledFn fn = nullptr;
-    static bool tried = false;
-    if (!tried) {
-        tried = true;
+    static const EncodeTiledFn fn = [] {
         void* p = nullptr;
         cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-            q == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeTiledFn>(p);
-    }
+        return cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess
+                   ? reinterpret_cast<EncodeTiledFn>(p)
+                   : nullptr;
+    }();
     return fn;
 }
 
@@ -86,6 +84,7 @@ struct mdc_ctx {
     bool plan_tma_ok = false;
     TileDesc* d_tiles = nullptr;
     int* d_counters = nullptr;   // ring of work counters (one per launch in flight)
+    cudaEvent_t counter_free[kCounterRing] = {};   // recorded behind the launch that used the slot last; its next user waits on it
     unsigned counter_next = 0;
     MapCache map_cache;                  // TMA descriptor sets (descriptors are passed to the kernel by value)
     // texture-gather loader: device limits, self-check verdict, cache of texture-object sets
@@ -282,6 +281,7 @@ int ctx_common_init(mdc_ctx* c, int device) {
     c->sm_count = v;
     CU_CHECK(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
     CU_CHECK(cudaMalloc(&c->d_counters, kCounterRing * sizeof(int)));
+    for (cudaEvent_t& ev : c->counter_free) CU_CHECK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
     CU_CHECK(cudaMalloc(&c->d_rc, kRcFxOffset * sizeof(double) + kGstepFxScratchBytes));
     const char* e = getenv("MDC_USE_TMA");
     if (e) c->use_tma = atoi(e);
@@ -540,7 +540,11 @@ int run_fused_staged(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frame
                      int cap_per_sm, int study, cudaStream_t stream, long long& launches) {
     FusedParams p;
     fused_params(p, c, d_frames, pitch, n_frames, u, outs, in_kernel);
-    p.work_counter = c->d_counters + (c->counter_next++ % kCounterRing);
+    // A counter is zeroed and then drawn from by the launch that takes it.  The launch that took the slot last may still run on
+    // another caller stream, so the zeroing waits for it; on one stream that wait is already satisfied.
+    const unsigned slot = c->counter_next++ % kCounterRing;
+    p.work_counter = c->d_counters + slot;
+    CU_CHECK(cudaStreamWaitEvent(stream, c->counter_free[slot], 0));
     CU_CHECK(cudaMemsetAsync(p.work_counter, 0, sizeof(int), stream));
     p.box_px_max = c->box_px_max;
     p.chunk_frames = c->chunk_frames > 0 ? c->chunk_frames : 48;
@@ -563,6 +567,7 @@ int run_fused_staged(mdc_ctx* c, const uint8_t* d_frames, int pitch, int n_frame
     if (study != kStudyAll && tma && u.vig && in_kernel == 1 && min_ctas == 3 && outs.type == MDC_OUT_F32)
         CU_CHECK(launch_fused_study(p, maps, grid, study, stream));
     else CU_CHECK(launch_fused(p, maps, grid, min_ctas, outs.type, stream));
+    CU_CHECK(cudaEventRecord(c->counter_free[slot], stream));
     launches++;
     return MDC_OK;
 }
@@ -794,6 +799,7 @@ extern "C" void mdc_ctx_destroy(mdc_ctx* c) {
     cudaFree(c->d_tiles); cudaFree(c->d_counters); cudaFree(c->d_rc);
     for (auto& s : c->map_cache.slots) free(s.set);
     cudaDeviceSynchronize();
+    for (cudaEvent_t ev : c->counter_free) if (ev) cudaEventDestroy(ev);
     for (auto& s : c->tex_cache.slots) tex_release(s);
     if (c->aux_stream) { cudaStreamDestroy(c->aux_stream); cudaEventDestroy(c->ev_fork); cudaEventDestroy(c->ev_join); }
     for (int s = 0; s < kHostPipeDepth; ++s) {

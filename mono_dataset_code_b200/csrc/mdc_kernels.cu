@@ -23,6 +23,7 @@
 #include <stdlib.h>
 
 #include <algorithm>
+#include <mutex>
 #include <type_traits>
 
 #include "mdc_atanf.h"
@@ -1760,6 +1761,7 @@ struct RmseOp {
 };
 
 static cudaEvent_t g_exposure_reader[64] = {};      // per device: recorded behind the last pass that read c_exposure_t
+static std::mutex g_exposure_mutex;                 // held from the wait on that event through its record (and over its creation)
 template <class Op>
 static cudaError_t launch_stream(const StreamArgs& a, const typename Op::Params& prm, cudaStream_t stream, int* grid_out = nullptr) {
     int dev = 0, sms = 132, per_sm = 0;
@@ -1799,7 +1801,11 @@ static cudaError_t launch_stream(const StreamArgs& a, const typename Op::Params&
     // exposure times -> constant memory (device-to-device, on this stream), behind the last pass that read the symbol
     cudaEvent_t* last_reader = g_exposure_reader;      // one event per device, shared by the three ops (they share the symbol)
     const bool use_const = a.n > 0 && a.n <= kEbMaxN && dev >= 0 && dev < 64;      // (no frames: nothing to copy, t may be null)
+    // The symbol is shared by every context and host thread: a pass that waited on the event before another one recorded it would
+    // overwrite the times that one's kernel still reads, so wait, copy, launch and record happen under one lock.
+    std::unique_lock<std::mutex> lock(g_exposure_mutex, std::defer_lock);
     if (use_const) {
+        lock.lock();
         if (!last_reader[dev] && (e = cudaEventCreateWithFlags(&last_reader[dev], cudaEventDisableTiming)) != cudaSuccess) return e;
         else if ((e = cudaStreamWaitEvent(stream, last_reader[dev], 0)) != cudaSuccess) return e;
         if ((e = cudaMemcpyToSymbolAsync(c_exposure_t, a.t, static_cast<size_t>(a.n) * sizeof(double), 0, cudaMemcpyDeviceToDevice, stream)) != cudaSuccess) return e;
